@@ -5,7 +5,7 @@
   python bench.py --impl reference --gpus N --steps K ...  # reference arm: the oracle port on the host CPU cores
 
 One step = one `simple_test` call = one frame pair -> one panoptic frame.  Prints ONE JSON line (rank 0).
-The headline (`value`, `e2e`, `roofline`) is measured in the PARITY precision "tc32" (fp32 activations, tcgen05 with split
+The headline (`value`, `e2e`, `roofline`) is measured in the PARITY precision "tc32" (fp32 activations, wgmma with split
 fp16 operands: label maps / ids identical to the oracle, tests/test_gpu_e2e.py, tests/test_gpu_fullsize.py); the bf16
 fast mode (one tensor-core pass, ~0.99 label agreement) is timed in the same run and reported under `fast_mode`.
   value      : pairs/s over ONE device-timed region (CUDA events) of K steps through the public clip loop
@@ -15,8 +15,8 @@ fast mode (one tensor-core pass, ~0.99 label agreement) is timed in the same run
                inside the timed region
   sequential_ms_per_pair : one pair at a time, L2 flushed in between (latency)
   next_rows  : the first rows past the hot path (SURVEY 8f): unified pan result, VPQ frame confusion
-  roofline   : the dominant kernel (tcgen05 implicit-GEMM conv, all launches of a step): algorithmic conv FLOPs /
-               summed kernel time, against the measured cuBLAS bf16 peak of MEASURED_PEAKS.json
+  roofline   : the dominant kernel (wgmma implicit-GEMM conv, all launches of a step): algorithmic conv FLOPs /
+               summed kernel time, against the measured cuBLAS bf16 peak of MEASURED_PEAKS.json (else the H100 SXM data sheet)
   cpu_baseline: the oracle (CPU port of the reference math) on a bounded sample, host cores
 """
 import argparse
@@ -46,7 +46,7 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sus=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sus=1400.0, src="fallback")
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sus=989.0, src="H100 SXM data sheet (dense bf16, 700 W)")
 
 
 class ClockSampler(threading.Thread):
@@ -227,6 +227,43 @@ def stock_pytorch_r50fpn(dev, H, W, flush):
     return out
 
 
+DUMP_MAX_BYTES = 64 << 20
+DUMP_SAMPLE = 1 << 19        # elements kept of a larger array: a fixed sample, np.random.default_rng(0) over its flat indices
+
+
+def dump_outputs(result, out_dir):
+    """Write every numeric array of one step's result (tensors and numpy arrays, nested in lists / tuples / dicts) as
+    out_dir/<path>.npy: integers up to 32 bits and floats as float32, 64-bit integers as float64.  An array of more than
+    DUMP_SAMPLE elements is replaced by the values at np.sort(default_rng(0).choice(size, DUMP_SAMPLE, replace=False)) of
+    its flattened form -- the same positions in every run, so two builds compare element for element."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = []
+
+    def walk(x, path):
+        if isinstance(x, torch.Tensor):
+            x = x.detach().cpu().numpy()
+        if isinstance(x, np.ndarray):
+            if x.dtype.kind in "biuf" and x.size:
+                arrays.append((path, x))
+        elif isinstance(x, dict):
+            for k in sorted(x, key=str):
+                walk(x[k], "%s.%s" % (path, k))
+        elif isinstance(x, (list, tuple)):
+            for i, v in enumerate(x):
+                walk(v, "%s.%d" % (path, i))
+
+    walk(result, "out")
+    total = 0
+    for path, a in arrays:
+        a = a.astype(np.float64 if a.dtype.itemsize == 8 and a.dtype.kind in "iu" else np.float32)
+        if a.size > DUMP_SAMPLE:
+            a = a.reshape(-1)[np.sort(np.random.default_rng(0).choice(a.size, DUMP_SAMPLE, replace=False))]
+        total += a.nbytes
+        if total > DUMP_MAX_BYTES:
+            raise SystemExit("bench.py: --dump-outputs would exceed %d bytes at %s" % (DUMP_MAX_BYTES, path))
+        np.save(os.path.join(out_dir, path + ".npy"), a)
+
+
 def run_gpu_arm(args):
     from vps_b200 import ops
     from vps_b200 import parallel as P
@@ -242,7 +279,7 @@ def run_gpu_arm(args):
     H, W = (1088, 1920) if viper else (args.height, args.width)
     det = build_product(args.precision, dev)
     det.label_dtype = torch.uint8                    # the reference's collector casts both maps to uint8 (test_vpq.py:52-56)
-    NPAIR = 4                                        # 4 distinct pairs = 201 MB of fp32 frames (> 126 MB L2)
+    NPAIR = 4                                        # 4 distinct pairs = 201 MB of fp32 frames (> 50 MB L2 of the H100)
     host = [(a.pin_memory(), b.pin_memory()) for a, b in synth_pairs(NPAIR, H, W, seed=100 + rank)]
     devp = [(a.to(dev), b.to(dev)) for a, b in host]
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
@@ -275,6 +312,7 @@ def run_gpu_arm(args):
     # viper: streaming clips -- the reference frame of frame t is frame t - 1 (cityscapes_vps.py:137-142), so the runner
     # reuses the previous pair's FPN features as reference features (results bit-identical: tests/test_gpu_e2e.py)
     runner = ClipRunner(det, dev, streaming=viper)
+    last = [None]                                    # the result of the last step of the latest region
 
     def region(n, offset, resident):
         src = devp if resident else host
@@ -295,6 +333,7 @@ def run_gpu_arm(args):
             chk += int(r[2]["panoptic_outputs"][0, 0, 0])       # the maps are host tensors here
         e.record()
         torch.cuda.synchronize()
+        last[0] = r
         return s.elapsed_time(e)
 
     # untimed: every CUDA-graph instance the timed regions replay must exist (2 ping-pong slots x {cached, uncached reference
@@ -309,6 +348,8 @@ def run_gpu_arm(args):
     l0 = ops.launch_count()
     ms = [region(args.steps, args.warmup + 5, True)]
     launches = ops.launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(last[0], args.dump_outputs)
     torch.cuda.synchronize()
     P.barrier()
     ms_e2e = [region(args.steps, args.warmup + 5 + args.steps, False)]
@@ -340,8 +381,8 @@ def run_gpu_arm(args):
         f_dev, f_e = [v / 1e3 for v in P.max_over_ranks([f_ms, f_e2e], dev)]
         fast = {"precision": "bf16", "value": world * args.steps / f_dev, "e2e": world * args.steps / f_e, "unit": "pairs/s",
                 "ms_per_step": 1e3 * f_dev / args.steps,
-                "parity": "bf16 operands, one tcgen05 pass: label agreement with the oracle 0.99 (semantic 0.9945 / panoptic 0.9896 "
-                          "at 1024x2048, tests/test_gpu_fullsize.py) -- lower precision than the reference, reported for context"}
+                "parity": "bf16 operands, one tensor-core pass: label agreement with the oracle checked by tests/test_gpu_fullsize.py "
+                          "-- lower precision than the reference, reported for context"}
         det.precision = args.precision
     # ---- SURVEY 8f rank 1 (the step after the path): get_unified_pan_result on the GPU, timed alone on a real result
     from vps_b200.postproc import PanUnifier
@@ -410,19 +451,12 @@ def run_gpu_arm(args):
         if tc_ms > 0:
             ach = tc_fl / (tc_ms * 1e-3) / 1e12
             passes = 3 if tc32 else 1
-            # DRAM traffic of the same kernels over one step, from the committed ncu pass (profiles/, see its README)
-            traffic = None
-            tp = os.path.join(ROOT, "profiles", "r2_dram_traffic.json")
-            if os.path.exists(tp):
-                try:
-                    traffic = json.load(open(tp)).get("tc32" if tc32 else "bf16")
-                except Exception:
-                    traffic = None
             roof = {"bound": "tensor",
                     "kernel": ("conv_igemm_tc32_kernel + dcn_igemm_tc32_kernel" if tc32 else "conv_igemm_tc_kernel + dcn_igemm_tc_kernel")
                               + " (all %d launches of a step)" % (tc_n // 2),
-                    "achieved": ach, "peak": pk["tf_sus"], "unit": "TFLOP/s", "frac": ach / pk["tf_sus"], "traffic": traffic,
-                    "peak_source": pk["src"] + " bf16_tflops_sustained (cuBLAS bf16, back to back)",
+                    "achieved": ach, "peak": pk["tf_sus"], "unit": "TFLOP/s", "frac": ach / pk["tf_sus"],
+                    "peak_source": pk["src"] if pk["src"] != "measured" else
+                                   "MEASURED_PEAKS.json bf16_tflops_sustained (cuBLAS bf16, back to back)",
                     "flops_per_step": tc_fl / 2, "ms_per_step": tc_ms / 2,
                     "tensor_passes": passes,
                     "tensor_pipe_frac": passes * ach / pk["tf_sus"],
@@ -440,7 +474,7 @@ def run_gpu_arm(args):
         bytes_out = 2 * H * W * det.label_dtype.itemsize
         line = {"metric": METRIC, "value": value, "unit": "pairs/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
                 "ms_per_step": 1e3 * t_dev / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-                "dtype": {"tc32": "f32 (tcgen05: 3 split-f16 products per MAC, fp32 accumulate promoted to RN register sums)",
+                "dtype": {"tc32": "f32 (wgmma: 3 split-f16 products per MAC, fp32 accumulate promoted to RN register sums)",
                           "bf16": "bf16", "fp32": "f32 (CUDA cores)"}[args.precision], "data": "synthetic",
                 "config": {"workload": ("VIPER-shape streaming inference, synthetic 30-frame 1088x1920 clips (1080 padded to 1088), " if viper else
                                         "FuseTrack inference, synthetic 2-frame %dx%d pair, " % (H, W)) +
@@ -450,7 +484,7 @@ def run_gpu_arm(args):
                                                  "(one ResNet-50-FPN pass per pair; algorithmic FLOPs still counted on the reference's "
                                                  "two-pass basis)") if viper else "off (independent pairs)",
                            "parallelism": "clip-sharded replicas x%d, no data-path collective" % world,
-                           "l2": "4 rotating input pairs (201 MB of fp32 frames > 126 MB L2) in both timed regions, steps are "
+                           "l2": "4 rotating input pairs (201 MB of fp32 frames > 50 MB L2) in both timed regions, steps are "
                                  "pipelined so no flush between them; sequential_ms_per_pair flushes 256 MiB between pairs",
                            "pipelining": "static part of pair i+1 (second CUDA-graph instance, side stream) overlaps pair i's "
                                          "tracker/mask/fusion tail; max(W,5) + 2 untimed runner steps precede the timed regions",
@@ -531,6 +565,8 @@ def main():
                     help="pairs = BASELINE config 2 (1024x2048 pairs); viper = config 4 (30-frame 1088x1920 clips, one per GPU)")
     ap.add_argument("--allow-short-warmup", action="store_true", help="profiling runs under ncu only (numbers are not bench values)")
     ap.add_argument("--profile-out", default="", help="write per-call device timings of one instrumented step (JSON lines)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the arrays the last timed step returned as DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if (args.impl == "b200" and not args.allow_short_warmup) else args.warmup
     if args.impl == "reference":

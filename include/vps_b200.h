@@ -1,5 +1,5 @@
 /*
- * vps_b200.h -- C ABI of libvps_b200.so (sm_100a kernels for the FuseTrack frame-pair path).
+ * vps_b200.h -- C ABI of libvps_b200.so (sm_90a kernels for the FuseTrack frame-pair path).
  *
  * Every entry point takes plain device pointers, sizes and a cudaStream_t (as void*), returns an
  * int status (0 = ok, negative = VPS_E_*), never throws across the ABI and never frees caller
@@ -23,7 +23,7 @@ extern "C" {
 #define VPS_OK 0
 #define VPS_E_ARG (-1)     /* bad argument / unsupported geometry */
 #define VPS_E_CUDA (-2)    /* a CUDA runtime / driver call failed (see vps_last_error) */
-#define VPS_E_NODEV (-3)   /* no sm_100 device */
+#define VPS_E_NODEV (-3)   /* no CUDA device */
 
 #define VPS_F32 0
 #define VPS_BF16 1
@@ -61,8 +61,8 @@ void vps_add_launch_count(int64_t n);
  * for oy < oh, ox < ow.  Out-of-range input taps read zero.  (oy_mul,oy_off,...) let a transposed
  * convolution run as stride-phase sub-convolutions writing interleaved output pixels.
  *
- * vps_conv2d_tc   : bf16 operands, fp32 accumulation on tcgen05 tensor cores (TMA im2col tiles,
- *                   accumulators in TMEM).  w = bf16 [cout_pad][kh*kw*cin_pad] (ci fastest,
+ * vps_conv2d_tc   : bf16 operands, fp32 accumulation on wgmma tensor cores (TMA im2col tiles,
+ *                   accumulators in registers).  w = bf16 [cout_pad][kh*kw*cin_pad] (ci fastest,
  *                   cin_pad = cin rounded up to cin_gran (64 or 16), cout_pad to 16), from vps_pack_weights_tc.
  *                   x must be VPS_BF16 with cs % 8 == 0 and 16-byte aligned ptr.
  * vps_conv2d_simt : fp32 (or bf16 storage) direct convolution on CUDA cores with fp32 FMA --
@@ -102,12 +102,13 @@ int64_t vps_packed_tc_bytes(int cout, int cin, int kh, int kw, int cin_gran);
 /* ---- fp32-parity tensor-core convolution ("tc32" precision) ------------------------------------
  * Same contract as vps_conv2d_tc, but x (and y, res) are fp32: the reference's convolutions are fp32 cuDNN calls
  * (resnet.py:506-517, flownet2.py:133-198, fpn.py:100-139 ...) and north_star asks for label maps / ids bit-exact.
- * Each operand is split on the fly into fp16(v) + bf16 corrections and three tcgen05 products
- *   fp16(a)*fp16(b) + bf16(a - fp16(a))*bf16(b) + bf16(a)*bf16(b - fp16(b))
- * are summed (~2^-21 relative per product, 3 tensor-core passes).  Because tcgen05.mma truncates when it adds into its
- * accumulator, the main product is accumulated in short chains that are promoted to round-to-nearest register sums
- * (conv_tc32.cu).  Weights are pre-split by vps_pack_weights_tc32 into [fp16 | bf16 | bf16] planes; the nprob stride
- * phases of a transposed convolution share ONE packed buffer (args[i].w identical, problem i = plane slice i).
+ * Each operand is split on the fly into A = fp16(v) and A2 = fp16(2^11 (v - A)), and three wgmma f16 products
+ *   A*B + 2^-11 (A2*B + A*B2)
+ * are summed (~2^-22 relative per operand, 3 tensor-core passes).  The tensor core's accumulation is not trusted to
+ * round to nearest over long chains, so every K step (32 channels) starts a fresh accumulator whose result is added into
+ * a round-to-nearest fp32 register sum (conv_tc32.cu).  Weights are pre-split by vps_pack_weights_tc32 into [B | B2]
+ * fp16 planes; the nprob stride phases of a transposed convolution share ONE packed buffer (args[i].w identical,
+ * problem i = plane slice i).
  * |value| > 65504 in x or w saturates the fp16 plane (the result then carries ~8 correct bits) and is counted:
  * vps_tc32_overflow(reset) returns the count (device sync) -- callers must treat non-zero as an error. */
 int vps_conv2d_tc32(const vps_conv_args* a, void* stream);
@@ -133,7 +134,7 @@ int vps_im2col(const vps_tensor* x, const vps_tensor* cols, int kh, int kw, int 
  * Optional fused LeakyReLU (FlowNetC.py:33,87).  f1,f2,out NHWC. */
 int vps_correlation(const vps_tensor* f1, const vps_tensor* f2, const vps_tensor* out, int pad,
                     int max_disp, int stride1, int stride2, int act, float slope, void* stream);
-/* the two implementations behind vps_correlation: banded GEMM on tcgen05 (bf16 features, C % 64 == 0, C <= 256,
+/* the two implementations behind vps_correlation: banded GEMM on wgmma (bf16 features, C % 64 == 0, C <= 256,
  * the (pad 20, d 20, s2 2) and (pad 4, d 4, s2 1) call sites) and the CUDA-core kernel (any dtype; parity mode). */
 int vps_correlation_tc(const vps_tensor* f1, const vps_tensor* f2, const vps_tensor* out, int pad,
                        int max_disp, int stride1, int stride2, int act, float slope, void* stream);

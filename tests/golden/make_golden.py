@@ -33,6 +33,17 @@ def weights_digest(sd):
     return h.hexdigest()
 
 
+def weights_fingerprint(sd):
+    """[n_tensors, 2] float64: sum |w| and sum w^2 of every tensor in key order.  The calibrated synthetic weights come out of
+    CPU convolutions whose last bits depend on the host's vector unit, so a bit-exact digest only holds on one machine type;
+    this fingerprint matches to ~1e-7 relative across hosts and still exposes any change of the generator or the init."""
+    rows = []
+    for k in sorted(sd.keys()):
+        w = sd[k].detach().cpu().double()
+        rows.append([float(w.abs().sum()), float((w * w).sum())])
+    return np.array(rows, np.float64)
+
+
 def main():
     oracle = make_model("C", 0)
     sd = oracle.state_dict()
@@ -46,7 +57,7 @@ def main():
     det.bbox_head.register_forward_hook(_first_cls)
     det.extra_neck.register_forward_hook(lambda m, i, o: cap.__setitem__("fused0", o[0].detach().clone()))
     img, ref = make_pair(H, W)
-    out = {"weights_sha256": np.array(weights_digest(sd)), "H": H, "W": W}
+    out = {"weights_sha256": np.array(weights_digest(sd)), "weights_fingerprint": weights_fingerprint(sd), "H": H, "W": W}
     with torch.no_grad():
         for f, (iid, a, b) in enumerate(((10001, img, ref), (10002, ref, img))):
             cap.clear()
@@ -64,7 +75,7 @@ def main():
             out["f%d_flow_full" % f] = cap["flow_full"].numpy().astype(np.float32)
             out["f%d_fcn_score" % f] = cap["fcn_score"].numpy().astype(np.float32)
             out["f%d_cls_score" % f] = cap["cls_score"].numpy().astype(np.float32)
-            out["f%d_fused0" % f] = cap["fused0"][:, ::16].numpy().astype(np.float32)   # every 16th channel
+            out["f%d_fused0" % f] = cap["fused0"][:, ::32].numpy().astype(np.float32)   # every 32nd channel (file < 1 MB)
     np.savez_compressed(OUT, **out)
     print("wrote", OUT, os.path.getsize(OUT) // 1024, "KiB")
 

@@ -1,13 +1,17 @@
 """CPU: the drop-in boundary -- registries, config loader, state_dict layout, C-ABI exports, no-fallback rule."""
 import ctypes
+import json
 import os
 import re
 
 import pytest
 import torch
 
+from tests.golden.ref_import import REF
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_CFG = "/root/reference/configs/cityscapes/fusetrack.py"
+REF_CFG = os.path.join(REF, "configs/cityscapes/fusetrack.py")       # REF: where the reference tree is (tests/golden/ref_import.py)
+REF_RECORD = os.path.join(ROOT, "tests", "golden", "reference_boundary.json")
 
 
 def test_registry_semantics_match_reference():
@@ -40,10 +44,21 @@ def test_all_reference_names_are_registered():
             assert reg.get(n) is not None, n
 
 
-@pytest.mark.skipif(not os.path.exists(REF_CFG), reason="reference tree not mounted")
+def _reference_record():
+    """the reference's fusetrack.py as its loader reads it and the contents of its registries, recorded from the reference
+    by tests/golden/make_boundary_golden.py"""
+    from tests.golden.make_boundary_golden import from_json
+    with open(REF_RECORD) as f:
+        return from_json(json.load(f))
+
+
 def test_reference_config_loads_unmodified_and_builds():
     from vps_b200 import Config, build_detector, fusetrack_cfg
-    cfg = Config.fromfile(REF_CFG)
+    rec = _reference_record()
+    if os.path.exists(REF_CFG):                  # where the reference tree is present, the record is still what it loads to
+        live = Config.fromfile(REF_CFG)
+        assert _plain(dict(live.model.items())) == rec["model"] and _plain(dict(live.test_cfg.items())) == rec["test_cfg"]
+    cfg = Config(dict(model=rec["model"], test_cfg=rec["test_cfg"]))
     assert hasattr(cfg.test_cfg, "flownet2") and not hasattr(cfg.test_cfg, "nope")
     assert cfg.test_cfg.rpn.nms_thr == 0.7 and cfg.model.bbox_head.num_classes == 9
     det = build_detector(cfg.model, train_cfg=None, test_cfg=cfg.test_cfg)
@@ -55,11 +70,42 @@ def test_reference_config_loads_unmodified_and_builds():
     assert det.class_mapping == {i: 10 + i for i in range(1, 9)}
 
 
-@pytest.mark.skipif(not os.path.exists(REF_CFG), reason="reference tree not mounted")
 def test_b200_classes_build_through_the_reference_registries():
-    """SURVEY 8b, second route: overwrite mmdet.models.registry.*.module_dict[name] with the B200 classes and build the
-    detector through the REFERENCE's own build_detector / build_from_cfg from the unmodified config.  Runs in a
-    subprocess: importing the reference on this mmcv-less CPU box needs process-wide stubs (tests/golden/ref_import.py)."""
+    """SURVEY 8b, second route: overwrite the reference's registries' module_dict[name] entries with this project's classes
+    and build the detector through those registries from the reference's config.  Everywhere: the reference's registries are
+    stood in for by registries that hold a placeholder class under every name, and with the defining module, that the
+    reference's own registries hold (recorded by tests/golden/make_boundary_golden.py); the detector is built by this
+    project's `build` on the stand-in DETECTORS registry.  Where the reference tree is present, additionally the same
+    through the reference's OWN registries and its own mmdet build_detector (in a subprocess: importing the reference on an
+    mmcv-less machine needs process-wide stubs, tests/golden/ref_import.py)."""
+    import types
+    from vps_b200.config import Config
+    from vps_b200.registry import Registry, build, install_into_reference
+    rec = _reference_record()
+    RR = types.SimpleNamespace()
+    for attr, names in rec["registries"].items():
+        reg = Registry(attr.lower())
+        for name, module in names.items():
+            reg.module_dict[name] = type(name, (object,), {"__module__": module})
+        setattr(RR, attr, reg)
+    ref_cls = RR.DETECTORS.get('PanopticFuseTrack')
+    assert ref_cls is not None and ref_cls.__module__.startswith('mmdet.')
+    done = install_into_reference(RR)
+    assert ('DETECTORS', 'PanopticFuseTrack') in done and ('BACKBONES', 'ResNet') in done and len(done) >= 12
+    for attr, name in done:
+        assert getattr(RR, attr).get(name).__module__.startswith('vps_b200.'), (attr, name)
+    cfg = Config(dict(model=rec["model"], test_cfg=rec["test_cfg"]))
+    cfg.model['pretrained'] = None
+    det = build(cfg.model, RR.DETECTORS, dict(train_cfg=None, test_cfg=cfg.test_cfg))
+    assert type(det).__module__ == 'vps_b200.detector', type(det)
+    for name in ('backbone', 'neck', 'extra_neck', 'panopticFPN', 'rpn_head', 'bbox_head', 'track_head', 'mask_head'):
+        assert type(getattr(det, name)).__module__.startswith('vps_b200.'), name
+    assert len(det.state_dict()) == 629
+    if os.path.exists(REF_CFG):
+        _build_through_the_live_reference()
+
+
+def _build_through_the_live_reference():
     import subprocess
     import sys
     code = r"""

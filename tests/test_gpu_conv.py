@@ -1,4 +1,4 @@
-"""GPU parity: convolution kernels (tcgen05 implicit GEMM and CUDA-core fp32) vs the oracle conv
+"""GPU parity: convolution kernels (wgmma implicit GEMM and CUDA-core fp32) vs the oracle conv
 (torch CPU fp32 F.conv2d / conv_transpose2d on the same seeded inputs)."""
 import pytest
 import torch

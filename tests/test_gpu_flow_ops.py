@@ -46,7 +46,7 @@ def test_resample2d_and_channelnorm(cuda):
 @pytest.mark.parametrize("cfg", [(20, 2, 256, 128, 256), (20, 2, 64, 37, 53), (4, 1, 256, 64, 96), (4, 1, 128, 21, 50),
                                  (20, 2, 192, 9, 11), (4, 1, 64, 3, 5)])
 def test_correlation_tensor_core(cuda, cfg):
-    """banded-GEMM correlation on tcgen05 vs the oracle on bf16-representable features (fp32 accumulation both)."""
+    """banded-GEMM correlation on wgmma vs the oracle on bf16-representable features (fp32 accumulation both)."""
     from oracle import ops as O
     from vps_b200 import ops
     md, s2, C, H, W = cfg

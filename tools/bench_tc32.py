@@ -1,5 +1,5 @@
 """Time and error of the tc32 convolution (vps_conv2d_tc32) per layer shape, next to the bf16 tensor-core and the fp32
-CUDA-core kernels.  VPS_TC32_GROUP=<K steps per in-tensor-core accumulation group> is read once per process.
+CUDA-core kernels.
 
     python tools/bench_tc32.py [--err] [--big]
 """
@@ -59,7 +59,6 @@ def run(shape, dtype, tc, reps=10):
 
 
 def main():
-    print("VPS_TC32_GROUP =", os.environ.get("VPS_TC32_GROUP", "(default)"))
     if "--err" in sys.argv:
         for shape in ERR_SHAPES:
             ms, tf, (x, wt, b, y, pad, s) = run(shape, torch.float32, True, reps=2)

@@ -1,7 +1,7 @@
 """Design experiment (CPU, test infrastructure): how many bf16 planes does the tensor-core parity mode need?
 
 Every dense contraction of the oracle (conv / conv_transpose / linear / DCN matmul / correlation / tracker dot) is
-replaced by the arithmetic a split-bf16 tcgen05 path performs: operands split into P bf16 planes
+replaced by the arithmetic a split-bf16 tensor-core path performs: operands split into P bf16 planes
 (x = x0 + x1 (+ x2), x_k = bf16(residual)), products x_i * w_j for i + j < P accumulated in fp32.  The clip of the
 e2e parity test is then compared with the unmodified fp32 oracle.
 

@@ -1,4 +1,4 @@
-"""vps_b200: Blackwell-native FuseTrack frame-pair path (drop-in modules for mcahny/vps's registries).
+"""vps_b200: Hopper-native FuseTrack frame-pair path (drop-in modules for mcahny/vps's registries).
 
     from vps_b200 import Config, build_detector
     cfg = Config.fromfile('<reference>/configs/cityscapes/fusetrack.py')      # loads unmodified

@@ -1,4 +1,4 @@
-"""Build libvps_b200.so (the C-ABI kernel library) in-tree with nvcc for sm_100a.
+"""Build libvps_b200.so (the C-ABI kernel library) in-tree with nvcc for sm_90a (H100).
 
 Incremental: each csrc/*.cu is compiled to build/*.o only when it (or a header) is newer than the
 object; objects are linked into vps_b200/lib/libvps_b200.so.  No GPU is needed (cross-compile).
@@ -15,7 +15,7 @@ LIBDIR = os.path.join(ROOT, "lib")
 LIB = os.path.join(LIBDIR, "libvps_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -69,7 +69,7 @@ def build(verbose=False, force=False):
         raise RuntimeError("vps_b200: CUDA build failed")
     objs = [os.path.join(OBJ, s[:-3] + ".o") for s in srcs]
     if force or jobs or _newer(objs, LIB):
-        cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a",
                                                       "-lcudart_static", "-Xlinker", "--no-undefined", "-lpthread",
                                                       "-ldl", "-lrt"]
         r = subprocess.run(cmd, capture_output=True, text=True)

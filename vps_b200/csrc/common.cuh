@@ -1,4 +1,4 @@
-// Shared device/host helpers for libvps_b200.so (sm_100a only).
+// Shared device/host helpers for libvps_b200.so (sm_90a).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>

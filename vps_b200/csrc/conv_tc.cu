@@ -1,45 +1,37 @@
-// Implicit-GEMM convolution on tcgen05 tensor cores (sm_100a).
+// Implicit-GEMM convolution on Hopper tensor cores (wgmma, sm_90a).
 //
 //   M = 128 output pixels (a th x tw patch of one image), N = block_n output channels (<= 256),
 //   K = kh*kw*cin_pad consumed 64 channels (=128 B, one SWIZZLE_128B row) per pipeline stage.
 //
-//   warp 0  : TMA producer.  The A tile of one (r,s,channel-chunk) K-step is ONE 4-D TMA box
-//             {64 ch, tw, th, 1} of the NHWC activation tensor, shifted by the filter tap; the
-//             tensor map's element strides implement the conv stride and TMA's out-of-bounds zero
-//             fill implements the padding -- im2col is never materialised.  B tile = 2-D box of the
-//             packed weights [cout_pad][K].
-//   warp 1  : allocates TMEM (512 columns = two fp32 accumulators of up to 256 columns) and issues
-//             tcgen05.mma (M=128, N=block_n, K=16) x4 per stage from one elected lane; tcgen05.commit
-//             releases smem stages and publishes finished accumulators.
-//   warps 2-5: epilogue.  tcgen05.ld the accumulator (thread = output pixel, 32 channels per load),
-//             bias + activation + residual + scale, convert, vectorised NHWC store (also into a
-//             channel slice of a concat buffer / interleaved pixels for transposed convs).
-//   Persistent: grid = #SMs, static round-robin over tiles, double-buffered accumulators so the
-//   epilogue of tile i overlaps the main loop of tile i+1.
+//   warp 0      : TMA producer.  The A tile of one (r,s,channel-chunk) K-step is ONE 4-D TMA box
+//                 {64 ch, tw, th, 1} of the NHWC activation tensor, shifted by the filter tap; the
+//                 tensor map's element strides implement the conv stride and TMA's out-of-bounds zero
+//                 fill implements the padding -- im2col is never materialised.  B tile = 2-D box of the
+//                 packed weights [cout_pad][K].
+//   warpgroups 1, 2: consumers, pixels 0-63 / 64-127 of the tile: wgmma (M=64, N=block_n, K=16) from shared memory into
+//                 register accumulators, one batch in flight while the previous one's ring slots are released; then bias +
+//                 activation + residual + scale, convert, NHWC store (also into a channel slice of a concat buffer /
+//                 interleaved pixels for transposed convs) straight from the accumulator fragments.
+//   Persistent: grid = #SMs, static round-robin over tiles; the producer runs ahead into the next tile during the epilogue.
 //
 // Replaces the cuDNN/cuBLAS calls behind every nn.Conv2d/ConvTranspose2d/Linear of the reference path.
 #include "conv_tc_common.cuh"
 
 namespace {
 
-constexpr int NUM_EPI_WARPS = 8;                      // 2 per TMEM lane quarter, alternating 32-column chunks
-constexpr int NUM_THREADS = 64 + 32 * NUM_EPI_WARPS;   // warp 0 = TMA, warp 1 = MMA, warps 2.. = epilogue
+constexpr int NUM_THREADS = 384;     // warpgroup 0: warp 0 = TMA producer (warps 1-3 idle); warpgroups 1, 2: MMA + epilogue
 
 
-// ---------------------------------------------------------------- single-issuer roles (warps 0 and 1)
-// Both run their loops warp-uniformly and pick the issuing lane with elect.sync: code under `if (lane == 0)` is
-// divergent to the compiler, which then wraps every TMA / tcgen05 instruction in a uniformity loop.  A lone warp
-// retires a dependent instruction every ~5 clk, so the per-step instruction count of these loops IS the pipeline
-// rate for small N (measured: 110 SASS instructions = 500 clk per K step): the loops are specialised on the mode
-// and, in halo mode, one barrier round covers a whole filter row (kw taps, 4*kw MMAs).
+// ---------------------------------------------------------------- TMA producer (warp 0)
+// The loop runs warp-uniformly and picks the issuing lane with elect.sync: code under `if (lane == 0)` is divergent to the
+// compiler, which then wraps every TMA instruction in a uniformity loop.  In halo mode one barrier round covers a whole
+// filter row (kw taps) when the row's weights fit one ring slot.
 struct Ring {
   uint32_t a_base, a_stage_bytes, b_base, b_stage_bytes, bar_base;
   __device__ __forceinline__ uint32_t afull(int s) const { return bar_base + 8u * s; }
   __device__ __forceinline__ uint32_t aempty(int s) const { return bar_base + 8u * (MAX_STAGES + s); }
   __device__ __forceinline__ uint32_t bfull(int s) const { return bar_base + 8u * (2 * MAX_STAGES + s); }
   __device__ __forceinline__ uint32_t bempty(int s) const { return bar_base + 8u * (3 * MAX_STAGES + s); }
-  __device__ __forceinline__ uint32_t tfull(int a) const { return bar_base + 8u * (4 * MAX_STAGES + a); }
-  __device__ __forceinline__ uint32_t tempty(int a) const { return bar_base + 8u * (4 * MAX_STAGES + 2 + a); }
 };
 
 // ---- halo mode: one activation box per channel chunk (A ring), weights per tap or per filter row (B ring)
@@ -138,138 +130,120 @@ __device__ __forceinline__ void producer_flat(const ConvTcParams& p, const Ring&
   if (STATS && lane == 0) { p.stats[blockIdx.x * 8 + 0] = st_a; p.stats[blockIdx.x * 8 + 1] = 0; }
 }
 
+// ---------------------------------------------------------------- consumer warpgroups (MMA + epilogue)
 // the (up to) four K16 MMAs of one tap: 64 channels = one SWIZZLE_128B row; +2 in the (addr >> 4) field = 32 bytes
-template <bool BK64>
-__device__ __forceinline__ void issue_tap(uint32_t d_tmem, uint64_t a_hi, uint64_t b_hi, uint32_t a_addr, uint32_t b_addr,
-                                          uint32_t idesc, int nk, uint32_t accumulate) {
-  const uint64_t adesc = a_hi | (uint64_t)((a_addr & 0x3FFFF) >> 4);
-  const uint64_t bdesc = b_hi | (uint64_t)((b_addr & 0x3FFFF) >> 4);
-  umma_bf16(d_tmem, adesc, bdesc, idesc, accumulate);
+template <int N, bool BK64>
+__device__ __forceinline__ void issue_tap(float (&d)[N / 2], uint64_t a_hi, uint64_t b_hi, uint32_t a_addr, uint32_t b_addr, int nk,
+                                          uint32_t& accumulate) {
+  const uint64_t adesc = desc_at(a_hi, a_addr), bdesc = desc_at(b_hi, b_addr);
+  wg::Mma<N, false>::run(d, adesc, bdesc, accumulate);
   if (BK64) {
-    if (nk > 1) umma_bf16(d_tmem, adesc + 2, bdesc + 2, idesc, 1u);
-    if (nk > 2) umma_bf16(d_tmem, adesc + 4, bdesc + 4, idesc, 1u);
-    if (nk > 3) umma_bf16(d_tmem, adesc + 6, bdesc + 6, idesc, 1u);
+    if (nk > 1) wg::Mma<N, false>::run(d, adesc + 2, bdesc + 2, 1u);
+    if (nk > 2) wg::Mma<N, false>::run(d, adesc + 4, bdesc + 4, 1u);
+    if (nk > 3) wg::Mma<N, false>::run(d, adesc + 6, bdesc + 6, 1u);
   }
+  accumulate = 1u;
 }
 
-template <bool ROWG, bool BK64, bool STATS>
-__device__ __forceinline__ void mma_halo(const ConvTcParams& p, const Ring& rg, uint32_t tmem_base, int lane) {
+// Ring slots are released one batch late: after batch i is committed, wgmma.wait_group 1 guarantees batch i - 1 has read
+// its operands, so its slots go back to the producer while batch i runs.  One elected thread per warpgroup arrives (the
+// empty barriers count both consumer warpgroups).
+struct Release {
+  int b = -1, a = -1;
+  __device__ __forceinline__ void flush(const Ring& rg, bool leader) {
+    if (leader) {
+      if (b >= 0) mbar_arrive(rg.bempty(b));
+      if (a >= 0) mbar_arrive(rg.aempty(a));
+    }
+    b = a = -1;
+  }
+};
+
+template <int N, bool BK64>
+__device__ __forceinline__ void consumer_tc(const ConvTcParams& p, const Ring& rg, int wg) {
   constexpr uint32_t row_bytes = BK64 ? 128u : 32u;
-  // instruction descriptor: D=f32, A=B=bf16, both K-major, N=block_n, M=128
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.block_n >> 3) << 17) |
-                         ((uint32_t)(BLOCK_M >> 4) << 24);
-  const int kw = p.kw, cin_chunks = p.cin_chunks, a_stages = p.a_stages, b_stages = p.b_stages;
-  const int ngrp = ROWG ? p.kh : p.kh * p.kw;
-  const int nk_last = p.nk_last;
-  const uint32_t halo_pitch = (uint32_t)p.halo_w * row_bytes;
-  const uint32_t tap_b_bytes = (uint32_t)p.block_n * row_bytes;
-  // descriptor high words are loop constants; the low word is (smem address >> 4)
-  const uint64_t a_hi = make_smem_desc(0, BK64 ? 64 : 16, halo_pitch);
-  const uint64_t b_hi = make_smem_desc(0, BK64 ? 64 : 16, 8u * row_bytes);
-  int as = 0, bs = 0, acc = 0;
-  uint32_t aphase = 0, bphase = 0, acc_phase = 0;
-  long long st_a = 0, st_b = 0, st_t = 0;
-  const long long t_begin = STATS ? clock64() : 0;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const int kw = p.kw, cin_chunks = p.cin_chunks, nk_last = p.nk_last;
+  const uint32_t tap_b_bytes = (uint32_t)N * row_bytes;
+  const uint64_t b_hi = desc_hi(row_bytes, 8u * row_bytes);
+  float d[N / 2];
+  int as = 0, bs = 0;
+  uint32_t aphase = 0, bphase = 0;
+  Release rel;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-    const long long t2 = STATS ? clock64() : 0;
-    mbar_wait(rg.tempty(acc), acc_phase ^ 1);
-    if (STATS) st_t += clock64() - t2;
-    tc_fence_after();
-    const uint32_t d_tmem = tmem_base + (uint32_t)acc * 256u;
-    uint32_t first = 0;
-    for (int cc = 0; cc < cin_chunks; ++cc) {
-      const int nk = cc == cin_chunks - 1 ? nk_last : 4;
-      const long long t0 = STATS ? clock64() : 0;
-      mbar_wait(rg.afull(as), aphase);
-      if (STATS) st_a += clock64() - t0;
-      uint32_t a_row = rg.a_base + as * rg.a_stage_bytes, a_tap = a_row;
-      const int a_cur = as;
-      int sx = 0;
-      if (++as == a_stages) { as = 0; aphase ^= 1; }
-      for (int g = 0; g < ngrp; ++g) {
-        const long long t1 = STATS ? clock64() : 0;
-        mbar_wait(rg.bfull(bs), bphase);
-        if (STATS) st_b += clock64() - t1;
-        tc_fence_after();
-        const uint32_t b_addr = rg.b_base + bs * rg.b_stage_bytes;
-        if (elect_one()) {
-          if (ROWG) {      // the kw taps of filter row g: A start moves one pixel (row_bytes) per tap
-            uint32_t at = a_row, bt = b_addr;
-            issue_tap<BK64>(d_tmem, a_hi, b_hi, at, bt, idesc, nk, first);
-            for (int j = 1; j < kw; ++j) {
-              at += row_bytes; bt += tap_b_bytes;
-              issue_tap<BK64>(d_tmem, a_hi, b_hi, at, bt, idesc, nk, 1u);
-            }
+    uint32_t accumulate = 0;
+    if (p.halo) {
+      // the 8 rows of an MMA row group are 8 pixels of one halo row; this warpgroup's 64 pixels start 8 halo rows down
+      const int ngrp = p.rowg ? p.kh : p.kh * kw;
+      const uint32_t halo_pitch = (uint32_t)p.halo_w * row_bytes;
+      const uint64_t a_hi = desc_hi(row_bytes, halo_pitch);
+      for (int cc = 0; cc < cin_chunks; ++cc) {
+        const int nk = cc == cin_chunks - 1 ? nk_last : 4;
+        mbar_wait(rg.afull(as), aphase);
+        uint32_t a_row = rg.a_base + as * rg.a_stage_bytes + (uint32_t)wg * 8u * halo_pitch, a_tap = a_row;
+        const int a_cur = as;
+        int sx = 0;
+        if (++as == p.a_stages) { as = 0; aphase ^= 1; }
+        for (int g = 0; g < ngrp; ++g) {
+          mbar_wait(rg.bfull(bs), bphase);
+          const uint32_t b_addr = rg.b_base + bs * rg.b_stage_bytes;
+          wg::fence();
+          if (p.rowg) {      // the kw taps of filter row g: A start moves one pixel (row_bytes) per tap
+            for (int j = 0; j < kw; ++j) issue_tap<N, BK64>(d, a_hi, b_hi, a_row + j * row_bytes, b_addr + j * tap_b_bytes, nk, accumulate);
           } else {
-            issue_tap<BK64>(d_tmem, a_hi, b_hi, a_tap, b_addr, idesc, nk, first);
+            issue_tap<N, BK64>(d, a_hi, b_hi, a_tap, b_addr, nk, accumulate);
           }
-          umma_commit(rg.bempty(bs));
-          if (g == ngrp - 1) umma_commit(rg.aempty(a_cur));
-        }
-        first = 1;
-        if (++bs == b_stages) { bs = 0; bphase ^= 1; }
-        if (ROWG) {
-          a_row += halo_pitch;
-        } else {          // next tap: one pixel to the right, or the start of the next halo row
-          a_tap += row_bytes;
-          if (++sx == kw) { sx = 0; a_row += halo_pitch; a_tap = a_row; }
+          wg::commit();
+          wg::wait<1>();
+          rel.flush(rg, leader);
+          rel.b = bs;
+          if (g == ngrp - 1) rel.a = a_cur;
+          if (++bs == p.b_stages) { bs = 0; bphase ^= 1; }
+          if (p.rowg) {
+            a_row += halo_pitch;
+          } else {          // next tap: one pixel to the right, or the start of the next halo row
+            a_tap += row_bytes;
+            if (++sx == kw) { sx = 0; a_row += halo_pitch; a_tap = a_row; }
+          }
         }
       }
+    } else {
+      // flat mode: gsub K steps per ring slot, operands of both kinds on the slot's `afull` barrier
+      const int ntaps = p.kh * kw, G = p.gsub;
+      const int T = cin_chunks * ntaps, q_last = T - ntaps;
+      const uint32_t a_box_bytes = (uint32_t)p.a_box_bytes;
+      const uint64_t a_hi = desc_hi(row_bytes, 8u * row_bytes);
+      for (int q0 = 0; q0 < T; q0 += G) {
+        const int cnt = min(G, T - q0);
+        mbar_wait(rg.afull(as), aphase);
+        const uint32_t a_slot = rg.a_base + as * rg.a_stage_bytes + (uint32_t)wg * 64u * row_bytes;
+        const uint32_t b_slot = rg.b_base + as * rg.b_stage_bytes;
+        wg::fence();
+        for (int j = 0; j < cnt; ++j)
+          issue_tap<N, BK64>(d, a_hi, b_hi, a_slot + j * a_box_bytes, b_slot + j * tap_b_bytes, q0 + j >= q_last ? nk_last : 4,
+                             accumulate);
+        wg::commit();
+        wg::wait<1>();
+        rel.flush(rg, leader);
+        rel.a = as;
+        if (++as == p.a_stages) { as = 0; aphase ^= 1; }
+      }
     }
-    if (elect_one()) umma_commit(rg.tfull(acc));
-    acc ^= 1;
-    if (acc == 0) acc_phase ^= 1;
-  }
-  if (STATS && lane == 0) {
-    p.stats[blockIdx.x * 8 + 2] = st_a; p.stats[blockIdx.x * 8 + 3] = st_b; p.stats[blockIdx.x * 8 + 4] = st_t;
-    p.stats[blockIdx.x * 8 + 5] = clock64() - t_begin;
+    wg::wait<0>();
+    wg::fence_regs(d);
+    rel.flush(rg, leader);
+    epi_frag<N>(p, d, tile, wg * 64);
   }
 }
 
-template <bool BK64, bool STATS>
-__device__ __forceinline__ void mma_flat(const ConvTcParams& p, const Ring& rg, uint32_t tmem_base, int lane) {
-  constexpr uint32_t row_bytes = BK64 ? 128u : 32u;
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.block_n >> 3) << 17) |
-                         ((uint32_t)(BLOCK_M >> 4) << 24);
-  const int stages = p.a_stages, G = p.gsub, ntaps = p.kh * p.kw;
-  const int T = p.cin_chunks * ntaps;
-  const int q_last = T - ntaps;                     // steps >= q_last belong to the last channel chunk
-  const int nk_last = p.nk_last;
-  const uint32_t a_box_bytes = (uint32_t)p.a_box_bytes, b_tile_bytes = (uint32_t)p.block_n * row_bytes;
-  const uint64_t a_hi = make_smem_desc(0, BK64 ? 64 : 16, 8u * row_bytes);
-  const uint64_t b_hi = a_hi;
-  int st = 0, acc = 0;
-  uint32_t phase = 0, acc_phase = 0;
-  long long st_a = 0, st_t = 0;
-  const long long t_begin = STATS ? clock64() : 0;
-  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-    const long long t2 = STATS ? clock64() : 0;
-    mbar_wait(rg.tempty(acc), acc_phase ^ 1);
-    if (STATS) st_t += clock64() - t2;
-    tc_fence_after();
-    const uint32_t d_tmem = tmem_base + (uint32_t)acc * 256u;
-    for (int q0 = 0; q0 < T; q0 += G) {
-      const int cnt = min(G, T - q0);
-      const long long t0 = STATS ? clock64() : 0;
-      mbar_wait(rg.afull(st), phase);
-      if (STATS) st_a += clock64() - t0;
-      tc_fence_after();
-      const uint32_t a_slot = rg.a_base + st * rg.a_stage_bytes, b_slot = rg.b_base + st * rg.b_stage_bytes;
-      if (elect_one()) {
-        for (int j = 0; j < cnt; ++j)
-          issue_tap<BK64>(d_tmem, a_hi, b_hi, a_slot + j * a_box_bytes, b_slot + j * b_tile_bytes, idesc,
-                          q0 + j >= q_last ? nk_last : 4, (uint32_t)((q0 + j) != 0));
-        umma_commit(rg.aempty(st));
-      }
-      if (++st == stages) { st = 0; phase ^= 1; }
-    }
-    if (elect_one()) umma_commit(rg.tfull(acc));
-    acc ^= 1;
-    if (acc == 0) acc_phase ^= 1;
-  }
-  if (STATS && lane == 0) {
-    p.stats[blockIdx.x * 8 + 2] = st_a; p.stats[blockIdx.x * 8 + 3] = 0; p.stats[blockIdx.x * 8 + 4] = st_t;
-    p.stats[blockIdx.x * 8 + 5] = clock64() - t_begin;
+template <bool BK64>
+__device__ __forceinline__ void consumer_tc_n(const ConvTcParams& p, const Ring& rg, int wg) {
+  switch (p.block_n) {
+    case 16: consumer_tc<16, BK64>(p, rg, wg); break;
+    case 32: consumer_tc<32, BK64>(p, rg, wg); break;
+    case 64: consumer_tc<64, BK64>(p, rg, wg); break;
+    case 128: consumer_tc<128, BK64>(p, rg, wg); break;
+    default: consumer_tc<256, BK64>(p, rg, wg); break;
   }
 }
 
@@ -286,55 +260,31 @@ conv_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
   const uint32_t b_stage_bytes = (uint32_t)p.block_n * row_bytes * (p.halo ? (p.rowg ? (uint32_t)p.kw : 1u) : (uint32_t)p.gsub);
   const uint32_t b_base = smem_base + (uint32_t)p.a_stages * a_stage_bytes;
   const uint32_t bar_base = b_base + (uint32_t)p.b_stages * b_stage_bytes;
-  // barrier slots (8 B each): afull, aempty, bfull, bempty [MAX_STAGES each], tmem_full[2], tmem_empty[2], tmem ptr
-  auto afull_bar = [&](int s) { return bar_base + 8u * s; };
-  auto aempty_bar = [&](int s) { return bar_base + 8u * (MAX_STAGES + s); };
-  auto bfull_bar = [&](int s) { return bar_base + 8u * (2 * MAX_STAGES + s); };
-  auto bempty_bar = [&](int s) { return bar_base + 8u * (3 * MAX_STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (4 * MAX_STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (4 * MAX_STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (4 * MAX_STAGES + 4);
-
-  const int warp = threadIdx.x >> 5;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);     // warp-uniform role index (wgmma issue is not treated as divergent)
   const int lane = threadIdx.x & 31;
-
-  // prologue on the critical path of every launch: one barrier per thread of warp 2 (36 inits), descriptors prefetched by
-  // warp 0, TMEM allocated by warp 1 -- all concurrently
-  if (warp == 2) {
-    if (lane < 4 * MAX_STAGES) mbar_init(bar_base + 8u * lane, 1);                    // afull / aempty / bfull / bempty
-    if (lane >= 28) {                                                               // lanes 28..31: tfull[0,1], tempty[0,1]
-      const int a = lane & 1;
-      if (lane < 30) mbar_init(tfull_bar(a), 1); else mbar_init(tempty_bar(a), 32 * NUM_EPI_WARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB0) : "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                 "r"((uint32_t)TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
-  // Programmatic dependent launch: everything above (barrier init, TMEM allocation, descriptor prefetch) overlaps the
-  // tail of the previous kernel in the stream; no global memory is touched before the wait.  Our own dependents are
-  // released immediately -- they block at their own wait until this grid has completed and flushed.
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-
   Ring rg;
   rg.a_base = smem_base; rg.a_stage_bytes = a_stage_bytes; rg.b_base = b_base; rg.b_stage_bytes = b_stage_bytes;
   rg.bar_base = bar_base;
-  const bool st = p.stats != nullptr;
+
+  // barrier slots (8 B each): afull, aempty, bfull, bempty [MAX_STAGES each]; full = one TMA arrival, empty = one arrival
+  // per consumer warpgroup
   if (warp == 0) {
-    // ===================== TMA producer =====================
+    mbar_init(bar_base + 8u * lane, (lane >> 3) & 1 ? 2 : 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  if (threadIdx.x == 32) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB0) : "memory");
+  }
+  __syncthreads();
+  // Programmatic dependent launch: the prologue above overlaps the tail of the previous kernel in the stream; no global
+  // memory is touched before the wait.  Our own dependents are released immediately -- they block at their own wait until
+  // this grid has completed and flushed.
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+
+  if (warp == 0) {
+    const bool st = p.stats != nullptr;
 #define VPS_ROLE(FN, ...) \
     do { if (st) FN<__VA_ARGS__, true>(p, rg, &tmA, &tmB0, &tmB1, &tmB2, &tmB3, lane); \
          else FN<__VA_ARGS__, false>(p, rg, &tmA, &tmB0, &tmB1, &tmB2, &tmB3, lane); } while (0)
@@ -342,35 +292,9 @@ conv_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
     else { if (st) producer_flat<true>(p, rg, &tmA, &tmB0, &tmB1, &tmB2, &tmB3, lane);
            else producer_flat<false>(p, rg, &tmA, &tmB0, &tmB1, &tmB2, &tmB3, lane); }
 #undef VPS_ROLE
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-#define VPS_MMA(FN, ...) \
-    do { if (st) FN<__VA_ARGS__, true>(p, rg, tmem_base, lane); else FN<__VA_ARGS__, false>(p, rg, tmem_base, lane); } while (0)
-    if (p.bk == 64) {
-      if (p.halo) { if (p.rowg) VPS_MMA(mma_halo, true, true); else VPS_MMA(mma_halo, false, true); }
-      else VPS_MMA(mma_flat, true);
-    } else {
-      if (p.halo) { if (p.rowg) VPS_MMA(mma_halo, true, false); else VPS_MMA(mma_halo, false, false); }
-      else VPS_MMA(mma_flat, false);
-    }
-#undef VPS_MMA
-  } else {
-    // ===================== epilogue (warps 2..9) =====================
-    switch (p.act) {
-      case VPS_ACT_RELU: epilogue_loop<VPS_ACT_RELU, NUM_EPI_WARPS / 4>(p, tmem_base, tfull_bar(0), tempty_bar(0), warp, lane); break;
-      case VPS_ACT_LRELU: epilogue_loop<VPS_ACT_LRELU, NUM_EPI_WARPS / 4>(p, tmem_base, tfull_bar(0), tempty_bar(0), warp, lane); break;
-      case VPS_ACT_SIGMOID: epilogue_loop<VPS_ACT_SIGMOID, NUM_EPI_WARPS / 4>(p, tmem_base, tfull_bar(0), tempty_bar(0), warp, lane); break;
-      default: epilogue_loop<VPS_ACT_NONE, NUM_EPI_WARPS / 4>(p, tmem_base, tfull_bar(0), tempty_bar(0), warp, lane); break;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"((uint32_t)TMEM_COLS)
-                 : "memory");
+  } else if (warp >= 4) {
+    if (p.bk == 64) consumer_tc_n<true>(p, rg, (warp - 4) >> 2);
+    else consumer_tc_n<false>(p, rg, (warp - 4) >> 2);
   }
 }
 
@@ -381,9 +305,11 @@ conv_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
 // so the 9x column matrix is never written to HBM.  K steps run chunk-major / tap-minor: for one 64-channel chunk the
 // nine taps of a tile touch the same ~(th+2) x (tw+2) x 128 B of input, which stays in L1.  Per tile the sampling
 // set-up of every (pixel, tap) -- 4 corner element offsets + 4 weights -- is computed once into shared memory.
-constexpr int DCN_GATHER_WARPS = 16;     // sampling is ALU-issue bound: 4 producer warps per SM sub-partition
-constexpr int DCN_EPI_WARPS = 4;
-constexpr int DCN_THREADS = 64 + 32 * DCN_EPI_WARPS + 32 * DCN_GATHER_WARPS;
+// 512 threads: warp 0 = weight TMA, warps 1-3 and 12-15 = sampling, warpgroups 1 and 2 = MMA + epilogue.  At 128 registers
+// per thread a consumer holds at most an N = 128 accumulator, so wider layers run as several N tiles.
+constexpr int DCN_GATHER_WARPS = 7;
+constexpr int DCN_THREADS = 512;
+constexpr int DCN_MAX_N = 128;
 constexpr int DCN_SETUP_BYTES = 9 * BLOCK_M * 32;
 
 struct DcnParams {
@@ -395,15 +321,13 @@ struct DcnParams {
 __device__ __forceinline__ void dcn_gather_loop(const ConvTcParams& p, const DcnParams& d, const Ring& rg, uint32_t setup_base,
                                                 int gtid) {
   const int stages = p.a_stages, cin_chunks = p.cin_chunks;
-  const int tiles_per_img = p.tiles_y * p.tiles_x;
   const int H = d.H, W = d.W;
   int st = 0;
   uint32_t phase = 0;
   const int j = gtid & 7;                    // 16-byte channel chunk of the 128-byte row
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-    const int img = tile / tiles_per_img;
-    const int rem = tile - img * tiles_per_img;
-    const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
+    const TileCoord tc = tile_coord(p, tile);
+    const int img = tc.img, ty = tc.ty, tx = tc.tx;
     // ---- sampling set-up of all (tap, pixel) pairs of this tile
     for (int item = gtid; item < 9 * BLOCK_M; item += 32 * DCN_GATHER_WARPS) {
       const int k = item >> 7, r = item & (BLOCK_M - 1);
@@ -440,9 +364,7 @@ __device__ __forceinline__ void dcn_gather_loop(const ConvTcParams& p, const Dcn
         mbar_wait(rg.aempty(st), phase ^ 1);
         const uint32_t a_slot = rg.a_base + st * rg.a_stage_bytes;
         constexpr int ROWS_PER_PASS = 32 * DCN_GATHER_WARPS / 8;       // 8 lanes (16-byte chunks) per pixel row
-#pragma unroll
-        for (int i = 0; i < BLOCK_M / ROWS_PER_PASS; ++i) {
-          const int r = (gtid >> 3) + ROWS_PER_PASS * i;
+        for (int r = gtid >> 3; r < BLOCK_M; r += ROWS_PER_PASS) {
           const uint32_t sa = setup_base + (uint32_t)(k * BLOCK_M + r) * 32u;
           float w0, w1, w2, w3;
           int o0, o1, o2, o3;
@@ -495,62 +417,44 @@ dcn_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmB, const ConvTcParams 
   rg.b_stage_bytes = (uint32_t)p.block_n * 128u;
   const uint32_t setup_base = rg.b_base + (uint32_t)p.a_stages * rg.b_stage_bytes;
   rg.bar_base = setup_base + DCN_SETUP_BYTES;
-  const uint32_t tmem_slot = rg.bar_base + 8u * (4 * MAX_STAGES + 4);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);     // warp-uniform role index (wgmma issue is not treated as divergent)
   if (threadIdx.x == 0) {
     for (int s = 0; s < MAX_STAGES; ++s) {
       mbar_init(rg.afull(s), 1 + 32 * DCN_GATHER_WARPS);     // weight TMA (expect_tx arrival) + every gather thread
-      mbar_init(rg.aempty(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(rg.tfull(a), 1);
-      mbar_init(rg.tempty(a), 32 * DCN_EPI_WARPS);
+      mbar_init(rg.aempty(s), 2);                            // one arrival per consumer warpgroup
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"((uint32_t)TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  if (warp == 0) {
-    // weight producer: one {64 ch, block_n, 1 tap} box per K step, completing on the step's `afull` barrier
-    const int stages = p.a_stages;
-    int st = 0;
-    uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      for (int cc = 0; cc < p.cin_chunks; ++cc) {
-        for (int k = 0; k < 9; ++k) {
-          mbar_wait(rg.aempty(st), phase ^ 1);
-          if (elect_one()) {
-            mbar_expect_tx(rg.afull(st), rg.b_stage_bytes);
-            tma_load_3d(rg.b_base + st * rg.b_stage_bytes, &tmB, rg.afull(st), cc * 64, 0, k);
+  if (warp >= 4 && warp < 12) {
+    if (p.block_n <= 64) consumer_tc<64, true>(p, rg, (warp - 4) >> 2);
+    else consumer_tc<DCN_MAX_N, true>(p, rg, (warp - 4) >> 2);
+  } else {
+    if (warp == 0) {
+      // weight producer: one {64 ch, block_n, 1 tap} box per K step, completing on the step's `afull` barrier
+      const int stages = p.a_stages;
+      int st = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        const int n0 = tile_coord(p, tile).n_idx * p.block_n;
+        for (int cc = 0; cc < p.cin_chunks; ++cc) {
+          for (int k = 0; k < 9; ++k) {
+            mbar_wait(rg.aempty(st), phase ^ 1);
+            if (elect_one()) {
+              mbar_expect_tx(rg.afull(st), rg.b_stage_bytes);
+              tma_load_3d(rg.b_base + st * rg.b_stage_bytes, &tmB, rg.afull(st), cc * 64, n0, k);
+            }
+            if (++st == stages) { st = 0; phase ^= 1; }
           }
-          if (++st == stages) { st = 0; phase ^= 1; }
         }
       }
+    } else {
+      dcn_gather_loop(p, d, rg, setup_base, warp < 4 ? (int)threadIdx.x - 32 : (int)threadIdx.x - 384 + 96);
     }
-  } else if (warp == 1) {
-    mma_flat<true, false>(p, rg, tmem_base, lane);
-  } else if (warp < 2 + DCN_EPI_WARPS) {
-    epilogue_loop<VPS_ACT_NONE, DCN_EPI_WARPS / 4>(p, tmem_base, rg.tfull(0), rg.tempty(0), warp, lane);
-  } else {
-    dcn_gather_loop(p, d, rg, setup_base, (int)threadIdx.x - 32 * (2 + DCN_EPI_WARPS));
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS) : "memory");
   }
 }
 
@@ -683,7 +587,7 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
   {
     const int64_t m_tiles = (int64_t)a->x.n * p.tiles_y * p.tiles_x * nprob;
     double best = -1.0;
-    for (int bn = 16; bn <= 256 && bn <= cout_pad; bn += 16) {
+    for (int bn = 16; bn <= 256 && bn <= cout_pad; bn *= 2) {     // the N extents the consumer is instantiated for
       if (cout_pad % bn) continue;
       const int64_t tiles = m_tiles * (cout_pad / bn);
       const double waves = (double)((tiles + g_num_sms - 1) / g_num_sms);
@@ -823,10 +727,11 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
     double m[8] = {0};
     for (int i = 0; i < grid; ++i) for (int j = 0; j < 8; ++j) m[j] += (double)h[i * 8 + j] / grid;
     const int tiles_cta = (p.total_tiles + grid - 1) / grid;
-    fprintf(stderr, "conv_tc stats %dx%d %d->%d @%dx%d halo=%d/%d g%d bn=%d bk=%d stages a%d b%d tiles/cta %d steps/tile %d | clk/CTA: total %.0f  "
-            "prod wait Aempty %.0f Bempty %.0f | mma wait Afull %.0f Bfull %.0f tmem-empty %.0f | epi wait tfull %.0f work %.0f\n",
+    // slots 0 / 1: the producer's clocks waiting for free A / B ring slots (the only role that records them)
+    fprintf(stderr, "conv_tc stats %dx%d %d->%d @%dx%d halo=%d/%d g%d bn=%d bk=%d stages a%d b%d tiles/cta %d steps/tile %d | clk/CTA: "
+            "prod wait Aempty %.0f Bempty %.0f\n",
             a->kh, a->kw, a->cin, a->cout, a->oh, a->ow, p.halo, p.rowg, p.gsub, block_n, bk, p.a_stages, p.b_stages, tiles_cta,
-            a->kh * a->kw * p.cin_chunks, m[5], m[0], m[1], m[2], m[3], m[4], m[6], m[7]);
+            a->kh * a->kw * p.cin_chunks, m[0], m[1]);
   }
   return VPS_OK;
 }
@@ -866,17 +771,19 @@ extern "C" int vps_deform_conv_tc(const vps_tensor* x, const vps_tensor* offset,
   }
   p.tw = best_tw; p.th = 128 / best_tw;
   p.tiles_x = vps::cdiv(x->w, p.tw); p.tiles_y = vps::cdiv(x->h, p.th);
-  p.n_tiles_n = 1; p.block_n = cout_pad;
+  // weight rows past cout_pad are TMA zero fill
+  p.block_n = cout_pad <= 64 ? 64 : DCN_MAX_N;
+  p.n_tiles_n = vps::cdiv(cout_pad, p.block_n);
   p.kh = p.kw = 3; p.sh = p.sw = 1; p.ph = p.pw = 1;
   p.cin_chunks = x->c / 64;
   p.gsub = 1; p.nk_last = 4; p.halo = 0; p.rowg = 0;
   p.a_box_bytes = BLOCK_M * 128; p.a_stage_bytes = p.a_box_bytes;
-  const int stage_bytes = p.a_stage_bytes + cout_pad * 128;
+  const int stage_bytes = p.a_stage_bytes + p.block_n * 128;
   int stages = (200 * 1024 - DCN_SETUP_BYTES) / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   VPS_CHECK_ARG(stages >= 2, "deform_conv_tc: ring does not fit");
   p.a_stages = p.b_stages = stages;
-  p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x;
+  p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
   p.total_tiles = p.tiles_per_prob;
   p.y = y->ptr; p.y_h = y->h; p.y_w = y->w; p.y_cs = y->cs; p.y_dtype = y->dtype;
   const int esz = y->dtype == VPS_BF16 ? 2 : 4;
@@ -894,7 +801,7 @@ extern "C" int vps_deform_conv_tc(const vps_tensor* x, const vps_tensor* offset,
     const cuuint64_t K = (cuuint64_t)9 * x->c;
     cuuint64_t dims[3] = {(cuuint64_t)x->c, (cuuint64_t)cout_pad, 9};
     cuuint64_t strides[2] = {K * 2, (cuuint64_t)x->c * 2};
-    cuuint32_t box[3] = {64, (cuuint32_t)cout_pad, 1};
+    cuuint32_t box[3] = {64, (cuuint32_t)p.block_n, 1};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = encode(&tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)w, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

@@ -1,24 +1,22 @@
-// Correlation (cost volume) on tcgen05 tensor cores -- the FlowNetC (pad 20, d 20, s2 2 -> 441 ch) and
+// Correlation (cost volume) on Hopper tensor cores (wgmma) -- the FlowNetC (pad 20, d 20, s2 2 -> 441 ch) and
 // LiteFlowNetCorr (pad 4, d 4, s2 1 -> 81 ch) call sites of correlation_cuda.forward
 // (correlation_cuda.cc:10-87, correlation_cuda_kernel.cu:74-147), bf16 features, fp32 accumulation.
 //
-// Banded GEMM, transposed on purpose:  D[n, m] = sum_c f2[n, c] * f1[m, c]
+// Banded GEMM:  D[n, m] = sum_c f2[n, c] * f1[m, c]
 //   m = one of 96 output pixels of a TH x TW tile (pixels of ONE stride2-parity class, so that every needed f2
 //       pixel has the same parity and element-strided TMA boxes fetch exactly the useful pixels),
-//   n = f2 pixels of the tile's displacement neighbourhood, (TH + 2R) rows x 32 columns, 4 rows (128 pixels = 128
-//       TMEM lanes) per MMA block.
-// With f2 on the TMEM-lane axis, a thread (lane = neighbourhood column j') that walks the accumulator columns of a
-// tile row i finds in column (i, j) the value of output pixel (i, j) at displacement (tj, ti) = (i' - i, j' - j):
-// consecutive lanes hold consecutive ti of the SAME output pixel, i.e. consecutive addresses of the NHWC output --
-// the band is extracted with plain coalesced stores, no shuffles and no shared-memory staging.
+//   n = f2 pixels of the tile's displacement neighbourhood, (TH + 2R) rows x 32 columns, 4 rows (128 pixels) per block;
+//       each consumer warpgroup multiplies 2 of those rows (M = 64, N = 96, K = 16).
+// Accumulator element (n, m) is output pixel m = (i, j) at displacement (tj, ti) = (i' - i, j' - j) for the
+// neighbourhood pixel n = (i', j'); the band is stored straight from the register fragments.
 //
-//   warp 0: TMA producer (f1 tile resident & double-buffered per tile; f2 blocks streamed through a 6-stage ring)
-//   warp 1: TMEM alloc + tcgen05.mma issue (M=128, N=96, K=16), accumulators double-buffered
-//   warps 2-9: epilogue, warp -> neighbourhood row 4*block + (warp % 4); the two warps of a row split the output rows
+//   warp 0         : TMA producer (f1 tile resident & double-buffered per tile; f2 blocks streamed through a 6-stage ring)
+//   warpgroups 1, 2: wgmma + band extraction
 #include <cudaTypedefs.h>
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
@@ -50,69 +48,112 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+// retry loop inside the PTX block (no divergent C++ loop or call between wgmma batches); traps after 2^26 failed polls
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0, spins = 0;
-  while (true) {
-    asm volatile(
-        "{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
-        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (done) break;
-    if (++spins > (1u << 26)) {
-      printf("vps corr_tc: mbarrier timeout block %d thread %d bar %u\n", blockIdx.x, threadIdx.x, bar);
-      __trap();
-    }
-  }
+  asm volatile(
+      "{\n.reg .pred p;\n.reg .u32 n;\nmov.u32 n, 0;\n"
+      "VPS_WAIT:\n"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+      "@p bra.uni VPS_DONE;\n"
+      "add.u32 n, n, 1;\n"
+      "setp.lt.u32 p, n, %2;\n"
+      "@p bra.uni VPS_WAIT;\n"
+      "trap;\n"
+      "VPS_DONE:\n}\n" ::"r"(bar), "r"(parity), "n"(1u << 26)
+      : "memory");
 }
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, int c3) {
   asm volatile(
       "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
       ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ uint64_t make_desc(uint32_t addr) {   // K-major, 128-byte rows, SWIZZLE_128B
-  uint64_t d = 0;
-  d |= (uint64_t)((addr & 0x3FFFF) >> 4);
+__device__ __forceinline__ uint64_t make_desc(uint32_t addr) {   // K-major, 128-byte rows, SWIZZLE_128B, 8-row groups 1 KiB apart
+  uint64_t d = (uint64_t)((addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-template <int N>
-__device__ __forceinline__ void tmem_ld(uint32_t taddr, uint32_t* r);
-template <>
-__device__ __forceinline__ void tmem_ld<4>(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(taddr) : "memory");
+
+// R = max_displacement / stride2, S2 = stride2.  TW = 32 - 2R so the neighbourhood is exactly 32 columns wide.
+template <int R, int S2, bool F16>
+__device__ __forceinline__ void corr_consumer(const CorrParams& p, uint32_t a_ring, uint32_t b_buf, uint32_t bars, int wg) {
+  constexpr int D = 2 * R + 1;
+  constexpr int TW = 32 - 2 * R;
+  constexpr int TH = NPIX / TW;
+  constexpr int NBLK = (TH + 2 * R) / 4;
+  auto afull = [&](int s) { return bars + 8u * s; };
+  auto aempty = [&](int s) { return bars + 8u * (A_STAGES + s); };
+  auto bfull = [&](int s) { return bars + 8u * (2 * A_STAGES + s); };
+  auto bempty = [&](int s) { return bars + 8u * (2 * A_STAGES + 2 + s); };
+  const bool leader = (threadIdx.x & 127) == 0;
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  const int tiles_per_par = p.tiles_y * p.tiles_x;
+  int stage = 0; uint32_t phase = 0;
+  int bsel = 0; uint32_t bphase = 0;
+  float d[NPIX / 2];
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    const int per_img = tiles_per_par * S2 * S2;
+    const int img = tile / per_img;
+    int t = tile - img * per_img;
+    const int par = t / tiles_per_par;
+    t -= par * tiles_per_par;
+    const int py = par / S2, px = par % S2;
+    const int y0 = (t / p.tiles_x) * TH * S2, x0 = (t % p.tiles_x) * TW * S2;
+    mbar_wait(bfull(bsel), bphase);
+    for (int b = 0; b < NBLK; ++b) {
+      for (int kc = 0; kc < p.kch; ++kc) {
+        mbar_wait(afull(stage), phase);
+        const uint64_t adesc = make_desc(a_ring + stage * A_BYTES + (uint32_t)wg * 64u * 128u);
+        const uint64_t bdesc = make_desc(b_buf + bsel * MAX_KCH * B_BYTES + kc * B_BYTES);
+        wg::fence();
+#pragma unroll
+        for (int k = 0; k < KC / 16; ++k)
+          wg::Mma<NPIX, F16>::run(d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)((kc | k) != 0));
+        wg::commit();
+        wg::wait<0>();
+        if (leader) mbar_arrive(aempty(stage));
+        if (++stage == A_STAGES) { stage = 0; phase ^= 1; }
+      }
+      wg::fence_regs(d);
+      // fragment element d[4q + 2h + e]: neighbourhood pixel n = 64 wg + 16 w + lane/4 + 8h, output pixel m = 8q + 2(lane%4) + e.
+      // The per-pixel index math below does not depend on the block; recomputing it here (opaque lane copy) keeps the
+      // compiler from hoisting ~100 values out of the block loop and spilling them.
+      int ln = lane;
+      asm volatile("" : "+r"(ln));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int n = 64 * wg + 16 * w + (ln >> 2) + 8 * h;
+        const int ip = 4 * b + (n >> 5), jp = n & 31;
+#pragma unroll
+        for (int q = 0; q < NPIX / 8; ++q) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int m = 8 * q + 2 * (ln & 3) + e;
+            const int i = m / TW, j = m - (m / TW) * TW;
+            const int tj = ip - i, ti = jp - j;
+            const int y = y0 + py + i * S2, x = x0 + px + j * S2;
+            if (tj >= 0 && tj < D && ti >= 0 && ti < D && y < p.H && x < p.W) {
+              float v = d[4 * q + 2 * h + e] * p.scale;
+              const int64_t o = (((int64_t)img * p.H + y) * p.W + x) * p.out_cs + tj * D + ti;
+              if (p.accumulate) v += ((const float*)p.out)[o];
+              if (p.act == VPS_ACT_LRELU) v = v > 0.f ? v : v * p.slope;
+              if (p.out_dtype == VPS_BF16) ((__nv_bfloat16*)p.out)[o] = __float2bfloat16_rn(v);
+              else ((float*)p.out)[o] = v;
+            }
+          }
+        }
+      }
+    }
+    if (leader) mbar_arrive(bempty(bsel));      // every MMA reading this f1 tile has completed
+    bsel ^= 1; if (bsel == 0) bphase ^= 1;
+  }
 }
-template <>
-__device__ __forceinline__ void tmem_ld<8>(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr) : "memory");
-}
-template <>
-__device__ __forceinline__ void tmem_ld<16>(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // R = max_displacement / stride2, S2 = stride2.  TW = 32 - 2R so the neighbourhood is exactly 32 columns wide.
 template <int R, int S2>
-__global__ void __launch_bounds__(320, 1)
+__global__ void __launch_bounds__(384, 1)
 corr_tc_kernel(const __grid_constant__ CUtensorMap tmF1, const __grid_constant__ CUtensorMap tmF2, const CorrParams p) {
-  constexpr int D = 2 * R + 1;
   constexpr int TW = 32 - 2 * R;
   constexpr int TH = NPIX / TW;
   constexpr int NBLK = (TH + 2 * R) / 4;
@@ -127,44 +168,28 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmF1, const __grid_constant__
   auto aempty = [&](int s) { return bars + 8u * (A_STAGES + s); };
   auto bfull = [&](int s) { return bars + 8u * (2 * A_STAGES + s); };
   auto bempty = [&](int s) { return bars + 8u * (2 * A_STAGES + 2 + s); };
-  auto tfull = [&](int s) { return bars + 8u * (2 * A_STAGES + 4 + s); };
-  auto tempty = [&](int s) { return bars + 8u * (2 * A_STAGES + 6 + s); };
-  const uint32_t tmem_slot = bars + 8u * (2 * A_STAGES + 8);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;     // warp-uniform role index
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < A_STAGES; ++s) { mbar_init(afull(s), 1); mbar_init(aempty(s), 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(bfull(s), 1); mbar_init(bempty(s), 1); mbar_init(tfull(s), 1); mbar_init(tempty(s), 256); }
+  if (threadIdx.x == 0) {      // full: one TMA arrival; empty: one arrival per consumer warpgroup
+    for (int s = 0; s < A_STAGES; ++s) { mbar_init(afull(s), 1); mbar_init(aempty(s), 2); }
+    for (int s = 0; s < 2; ++s) { mbar_init(bfull(s), 1); mbar_init(bempty(s), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(256u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
 
   const int tiles_per_par = p.tiles_y * p.tiles_x;
-  auto decode = [&](int tile, int& img, int& py, int& px, int& y0, int& x0) {
-    const int per_img = tiles_per_par * S2 * S2;
-    img = tile / per_img;
-    int t = tile - img * per_img;
-    const int par = t / tiles_per_par;
-    t -= par * tiles_per_par;
-    py = par / S2; px = par % S2;
-    y0 = (t / p.tiles_x) * TH * S2; x0 = (t % p.tiles_x) * TW * S2;
-  };
-
   if (warp == 0) {
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
       int bsel = 0; uint32_t bphase = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        int img, py, px, y0, x0;
-        decode(tile, img, py, px, y0, x0);
+        const int per_img = tiles_per_par * S2 * S2;
+        const int img = tile / per_img;
+        int t = tile - img * per_img;
+        const int par = t / tiles_per_par;
+        t -= par * tiles_per_par;
+        const int py = par / S2, px = par % S2;
+        const int y0 = (t / p.tiles_x) * TH * S2, x0 = (t % p.tiles_x) * TW * S2;
         // f1 tile (MMA B operand): resident for the whole tile, double-buffered across tiles
         mbar_wait(bempty(bsel), bphase ^ 1);
         mbar_expect_tx(bfull(bsel), b_tile_bytes);
@@ -183,104 +208,10 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmF1, const __grid_constant__
         bsel ^= 1; if (bsel == 0) bphase ^= 1;
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t fmt = p.f16 ? 0u : ((1u << 7) | (1u << 10));       // A / B format: 0 = f16, 1 = bf16
-      const uint32_t idesc = (1u << 4) | fmt | ((uint32_t)(NPIX >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      int stage = 0; uint32_t phase = 0;
-      int bsel = 0; uint32_t bphase = 0;
-      int acc = 0; uint32_t aphase = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        mbar_wait(bfull(bsel), bphase);
-        tc_fence_after();
-        for (int b = 0; b < NBLK; ++b) {
-          mbar_wait(tempty(acc), aphase ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + (uint32_t)acc * 128u;
-          for (int kc = 0; kc < p.kch; ++kc) {
-            mbar_wait(afull(stage), phase);
-            tc_fence_after();
-            const uint64_t adesc = make_desc(a_ring + stage * A_BYTES);
-            const uint64_t bdesc = make_desc(b_buf + bsel * MAX_KCH * B_BYTES + kc * B_BYTES);
-#pragma unroll
-            for (int k = 0; k < KC / 16; ++k)
-              umma_bf16(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (uint32_t)((kc | k) != 0));
-            umma_commit(aempty(stage));
-            if (++stage == A_STAGES) { stage = 0; phase ^= 1; }
-          }
-          umma_commit(tfull(acc));
-          acc ^= 1; if (acc == 0) aphase ^= 1;
-        }
-        umma_commit(bempty(bsel));      // all MMAs reading this f1 tile have completed when this fires
-        bsel ^= 1; if (bsel == 0) bphase ^= 1;
-      }
-    }
-  } else {
-    // 8 epilogue warps: warp -> TMEM lane quarter q (= neighbourhood row inside the block); the two warps of a quarter
-    // take alternate output rows i.  The TMEM load of the next row is in flight while the current one is stored.
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    int acc = 0; uint32_t aphase = 0;
-    const float inv_c = p.scale;
-    auto load_row = [&](uint32_t t_row, int i, uint32_t* r) {
-      if constexpr (TW == 12) { tmem_ld<8>(t_row + i * TW, r); tmem_ld<4>(t_row + i * TW + 8, r + 8); }
-      else { tmem_ld<16>(t_row + i * TW, r); tmem_ld<8>(t_row + i * TW + 16, r + 16); }
-    };
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      int img, py, px, y0, x0;
-      decode(tile, img, py, px, y0, x0);
-      for (int b = 0; b < NBLK; ++b) {
-        mbar_wait(tfull(acc), aphase);
-        tc_fence_after();
-        const int ip = 4 * b + q;        // neighbourhood row i' of this warp; lane = neighbourhood column j'
-        const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * 128u;
-        // output rows i with 0 <= i' - i < D, split between the two warps of this quarter
-        const int i_lo = max(0, ip - D + 1) + half, i_hi = min(TH - 1, ip);
-        auto store_row = [&](int i, const uint32_t* r) {
-          const int tj = ip - i;
-          const int y = y0 + py + i * S2;
-          if (y >= p.H) return;
-          const int64_t rowb = ((int64_t)img * p.H + y) * p.W * p.out_cs + tj * D + lane;
-#pragma unroll
-          for (int j = 0; j < TW; ++j) {
-            const int ti = lane - j;
-            const int x = x0 + px + j * S2;
-            if (ti >= 0 && ti < D && x < p.W) {
-              float v = __uint_as_float(r[j]) * inv_c;
-              const int64_t o = rowb + (int64_t)x * p.out_cs - j;
-              if (p.accumulate) v += ((const float*)p.out)[o];
-              if (p.act == VPS_ACT_LRELU) v = v > 0.f ? v : v * p.slope;
-              if (p.out_dtype == VPS_BF16) ((__nv_bfloat16*)p.out)[o] = __float2bfloat16_rn(v);
-              else ((float*)p.out)[o] = v;
-            }
-          }
-        };
-        uint32_t ra[TW], rb[TW];
-        int i = i_lo;
-        if (i <= i_hi) load_row(t_row, i, ra);
-        while (i <= i_hi) {
-          tmem_wait();
-          if (i + 2 <= i_hi) load_row(t_row, i + 2, rb);
-          store_row(i, ra);
-          i += 2;
-          if (i > i_hi) break;
-          tmem_wait();
-          if (i + 2 <= i_hi) load_row(t_row, i + 2, ra);
-          store_row(i, rb);
-          i += 2;
-        }
-        tmem_wait();
-        tc_fence_before();
-        mbar_arrive(tempty(acc));
-        acc ^= 1; if (acc == 0) aphase ^= 1;
-      }
-    }
+  } else if (warp >= 4) {
+    if (p.f16) corr_consumer<R, S2, true>(p, a_ring, b_buf, bars, (warp - 4) >> 2);
+    else corr_consumer<R, S2, false>(p, a_ring, b_buf, bars, (warp - 4) >> 2);
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 1)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u) : "memory");
 }
 
 PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
@@ -339,7 +270,7 @@ int launch(const vps_tensor* f1, const vps_tensor* f2, const vps_tensor* out, in
     attr_set = true;
   }
   const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
-  kern<<<grid, 320, smem, st>>>(tm1, tm2, p);
+  kern<<<grid, 384, smem, st>>>(tm1, tm2, p);
   VPS_CUDA_LAST("corr_tc_kernel");
   return VPS_OK;
 }
@@ -383,7 +314,7 @@ extern "C" int64_t vps_correlation_tc32_ws_bytes(const vps_tensor* f1) {
 // (v = hi + 2^-11 lo) and the banded GEMM runs three times, hi.hi, then hi.lo and lo.hi scaled by 2^-11 and accumulated
 // into the fp32 output (the activation is applied by the last pass).  Unlike the stacked convolutions a correlation is a
 // single K = C <= 256 contraction (16 MMAs per accumulator chain) whose result is not fed through further layers of the same
-// kind, so the tensor core's truncating accumulation (~3e-7 relative over such a chain) needs no promotion here.
+// kind, so the accumulation inside the tensor core needs no promotion here.
 // `ws`: vps_correlation_tc32_ws_bytes() of scratch, 256-byte aligned.  Same supported geometries as vps_correlation_tc.
 extern "C" int vps_correlation_tc32(const vps_tensor* f1, const vps_tensor* f2, const vps_tensor* out, int pad, int max_disp,
                                     int stride1, int stride2, int act, float slope, void* ws, void* stream) {

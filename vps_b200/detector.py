@@ -1,4 +1,4 @@
-"""PanopticFuseTrack on B200 -- the detector class the reference registers in DETECTORS
+"""PanopticFuseTrack on H100 -- the detector class the reference registers in DETECTORS
 (mmdet/models/detectors/panoptic_fusetrack.py:24-606), inference path.
 
 Construction follows TwoStageDetector.__init__ (two_stage.py:15-69): sub-modules are built from the
@@ -10,7 +10,7 @@ names, so `state_dict()` keys match a reference checkpoint.  Differences by desi
     (NMS mask download, MaskROI numpy, MaskRemoval numpy/cv2, SegTerm numpy, tracker loops) are kernels.
     Two 4-byte counters (number of detections, tracker memory size) are read back per frame to size the
     data-dependent launches.
-  * `precision`: "tc32" (fp32 activations, tcgen05 tensor cores with split operands: tf32 + two bf16 correction
+  * `precision`: "tc32" (fp32 activations, wgmma tensor cores with split operands: fp16 main + two fp16 correction
     products per K slab -- the parity mode, label maps / ids bit-exact vs the oracle), "bf16" (bf16 activations, one
     tensor-core pass: fastest, ~1e-2 relative on features) or "fp32" (CUDA-core fp32 FMA: debugging reference).
 """
@@ -191,7 +191,7 @@ class PanopticFuseTrack(nn.Module):
         _, _, H, W = img.shape
         dt = self.act_dtype
         # ResNet-50-FPN does not depend on the flow: it runs as a parallel branch (side stream / parallel graph branch), so
-        # the many launches that cannot fill 148 SMs on either side overlap with the other side's kernels
+        # the many launches that cannot fill 132 SMs on either side overlap with the other side's kernels
         br = ops.Branch("r50fpn")
         if br.side is None:
             ops.SCOPE[0] = 'flownet2'

@@ -1,10 +1,10 @@
-"""B200 FlowNet2 (frozen optical-flow sub-network of PanopticFuseTrack).
+"""vps_b200 FlowNet2 (frozen optical-flow sub-network of PanopticFuseTrack).
 
 Mirrors mmdet/models/flow_modules/{flownet2.py:32-198, FlowNetC.py:13-128, FlowNetS.py:15-94,
 FlowNetSD.py:11-106, FlowNetFusion.py:11-67, submodules.py:7-38}: same sub-module and parameter names
 (`flownetc.conv1.0.weight`, `flownets_1.deconv5.0.weight`, ...), inference (eval) dataflow only.
 
-B200 design points: every torch.cat of the reference is a pre-allocated NHWC concat buffer whose
+Design points: every torch.cat of the reference is a pre-allocated NHWC concat buffer whose
 producers write their channel slice directly (conv epilogues, transposed-conv phase kernels, the
 correlation kernel); ConvTranspose2d(4,2,1) runs as four stride-phase 2x2 convolutions on the
 tensor-core kernel; `x*div_flow`, `x/div_flow` scalings are folded into the resize kernels; warping

@@ -1,6 +1,6 @@
 """Layer helpers built on the C-ABI kernels: packed convolutions, transposed convolutions as
 stride-phase sub-convolutions, linear layers.  Precision follows the activation dtype:
-bf16 activations -> tcgen05 tensor-core kernel, fp32 activations -> fp32 CUDA-core kernel (parity mode).
+bf16 activations -> wgmma tensor-core kernel, fp32 activations -> fp32 CUDA-core kernel (parity mode).
 """
 import torch
 

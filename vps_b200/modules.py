@@ -1,4 +1,4 @@
-"""B200 modules registered under the reference's registry names (the host-side mirror of the
+"""vps_b200 modules registered under the reference's registry names (the host-side mirror of the
 reference's plugin interface for the FuseTrack path).
 
 Every class takes the constructor kwargs of its reference namesake (configs/cityscapes/fusetrack.py:2-86),

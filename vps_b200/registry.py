@@ -7,10 +7,10 @@ entry (registered name or a class), fills in `default_args` where the config is 
 mmdet/models/registry.py:3-11 names the nine registries; mmdet/models/builder.py:9-45 the build_* helpers
 (`build_detector` injects train_cfg / test_cfg, a list of configs becomes an nn.Sequential).
 
-The B200 modules register under the reference's own class names, so configs/cityscapes/fusetrack.py resolves unmodified
+The vps_b200 modules register under the reference's own class names, so configs/cityscapes/fusetrack.py resolves unmodified
 here.  `install_into_reference()` is the other integration route SURVEY 8b names: it overwrites the entries of the
-REFERENCE's registries (mmdet.models.registry.*.module_dict[name]) with the B200 classes, after which the reference's own
-`build_detector` builds the B200 detector from the unmodified config (tests/test_boundary.py).
+REFERENCE's registries (mmdet.models.registry.*.module_dict[name]) with the vps_b200 classes, after which the reference's own
+`build_detector` builds the vps_b200 detector from the unmodified config (tests/test_boundary.py).
 """
 from torch import nn
 
@@ -109,7 +109,7 @@ def build_detector(cfg, train_cfg=None, test_cfg=None):
 
 
 def install_into_reference(ref_registry_module):
-    """Overwrite the reference's registry entries with the B200 classes of the same name.
+    """Overwrite the reference's registry entries with the vps_b200 classes of the same name.
 
     ref_registry_module: the imported `mmdet.models.registry` (it holds BACKBONES ... DETECTORS).  Returns the list of
     (registry, class name) pairs that were replaced or added.  The reference's `register_module` refuses duplicates

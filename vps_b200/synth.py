@@ -1,5 +1,5 @@
 """Deterministic synthetic weight sets for any module tree with the reference's PanopticFuseTrack state_dict
-layout (the oracle model and the B200 detector share it).  There are no trained checkpoints offline
+layout (the oracle model and the vps_b200 detector share it).  There are no trained checkpoints offline
 (download_weights.sh needs the network); these sets exercise every code path (SURVEY.md 8d):
 
   "A": the reference's init rules (kaiming / xavier / normal as cited in SURVEY A.13).  bn3.gamma = 0
