@@ -30,10 +30,22 @@ SHAPES = [
     (1, 64, 64, 512, 1024, 3, 2, 0, "FlowNetSD 3x3 s2"),
     (1, 82, 16, 1024, 2048, 3, 1, 0, "Fusion conv0"),
     (1, 12, 64, 512, 1024, 4, 1, 0, "stem (s2d form)"),
+    (1, 48, 64, 512, 1024, 4, 1, 0, "FlowNetSD stem (s2d form)"),
+    (1, 162, 32, 512, 1024, 3, 1, 0, "Fusion conv1 162->32"),
+    (1, 6, 64, 1024, 2048, 3, 1, 0, "FlowNetSD conv0 6->64"),
+    (1, 11, 64, 1024, 2048, 3, 1, 0, "Fusion 11->64"),
+    (1, 256, 18, 256, 512, 3, 1, 0, "tap head 256->18"),
     (1, 16, 2, 1024, 2048, 3, 1, 0, "predict_flow full res"),
     (1, 194, 2, 256, 512, 3, 1, 0, "predict_flow2"),
     (1, 1024, 2, 16, 32, 3, 1, 0, "predict_flow6"),
     (1, 1024, 1024, 16, 32, 3, 1, 0, "conv6_1"),
+]
+# ConvTranspose2d(4, 2, 1) as four 2x2 stride-phase problems in one launch: n, cin, cout, in_h, in_w, note
+DECONVS = [
+    (1, 162, 16, 512, 1024, "Fusion deconv 162->16"),
+    (1, 386, 64, 128, 256, "FlowNet deconv 386->64"),
+    (1, 128, 32, 256, 512, "Fusion deconv 128->32"),
+    (1, 770, 128, 64, 128, "FlowNet deconv 770->128"),
 ]
 flush = None
 
@@ -83,6 +95,21 @@ def main():
               (note, k, k, s, cin, cout, oh, ow, n, ms, fl / ms / 1e9, by / 1e6, by / HBM_GBPS / 1e6, by / HBM_GBPS / 1e6 / ms),
               flush=True)
         del x, y, r, pk
+    from vps_b200.layers import deconv4x4_s2
+    for (n, cin, cout, h, w, note) in DECONVS:
+        if only and only not in note:
+            continue
+        g = torch.Generator().manual_seed(1)
+        x = empty_nhwc(n, h, w, cin, torch.float32, dev)
+        x.copy_(torch.randn(n, h, w, cin, generator=g).to(dev))
+        layer = deconv4x4_s2((torch.randn(cin, cout, 4, 4, generator=g) / (cin * 4) ** 0.5).to(dev),
+                             torch.randn(cout, generator=g).to(dev))
+        y = empty_nhwc(n, 2 * h, 2 * w, cout, torch.float32, dev)
+        ms = timeit(lambda: layer(x, y, act=ops.ACT_LRELU), iters)
+        fl = 2.0 * n * h * w * cout * cin * 16
+        print("%-28s 2x2 x4 phases %4d->%4d @%dx%d n%d: %.4f ms  %6.1f TF/s alg" % (note, cin, cout, h, w, n, ms, fl / ms / 1e9),
+              flush=True)
+        del x, y, layer
     if "--dcn" in sys.argv:
         for (h, w) in [(256, 512), (128, 256), (64, 128)]:
             for (ci, co) in [(256, 256), (256, 128), (128, 128)]:

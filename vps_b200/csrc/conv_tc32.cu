@@ -22,14 +22,18 @@
 //     main product A*B is added on top -- a chain of 2 main MMAs;
 //   * that step result is promoted into a per-thread register sum with a round-to-nearest fp32 add.
 //
-// Pipeline per CTA (persistent, one 128-pixel x block_n (<= 128) tile at a time, K consumed 32 channels per step):
+// Pipeline per CTA (persistent, one (64 * NWG)-pixel x block_n tile at a time, K consumed 32 channels per step):
 //   warp 0          : TMA producer: raw fp32 activation boxes {32 ch, pixels} into a staging ring; pre-split weight tiles
 //                     [B | B2] (vps_pack_weights_tc32) into the B ring.
 //   warps 1-3       : converters: staging box -> two SWIZZLE_64B operand planes A, A2 (generic-proxy writes ->
 //                     fence.proxy.async -> mbarrier).  In halo mode (stride 1, > 1 tap) one converted (th+kh-1) x (tw+kw-1)
 //                     box feeds all kh*kw taps through shifted descriptor start addresses.
-//   warpgroups 1, 2 : consumers, pixels 0-63 / 64-127: wgmma.kind f16 (M64 x N x K16) into registers, promotion, then bias /
-//                     activation / residual and the NHWC store straight from the accumulator fragments.
+//   warpgroups 1..NWG: consumers, pixels 64 wg .. 64 wg + 63: wgmma.kind f16 (M64 x N x K16) into registers, promotion, then
+//                     bias / activation / residual and the NHWC store straight from the accumulator fragments.
+// NWG = 2 (384 threads, block_n <= 128) or 4 (640 threads, block_n <= 64).  A K step is two dependent wgmma round trips
+// (the promotion order above), so a warpgroup spends a fixed few hundred clocks per step whatever N is; at N <= 64 four
+// warpgroups overlap those round trips and share each converted box and weight tile among twice the pixels.  At 640
+// threads the register cap is 96, which holds the N = 64 step accumulator + sum.  vps_conv2d_tc32_plan picks NWG.
 #include <cuda_fp16.h>
 
 #include "conv_tc_common.cuh"
@@ -37,9 +41,11 @@
 namespace {
 
 constexpr int T32_CONV_WARPS = 3;           // warps 1..3 (warp 0 = TMA)
-constexpr int T32_THREADS = 384;            // warpgroup 0: producer + converters; warpgroups 1, 2: consumers
 constexpr int T32_KC = 32;                  // channels per K step: 64-byte operand rows (SWIZZLE_64B), 2 x K16
 constexpr int T32_MAX_N = 128;              // step accumulator + promoted sum: 2 x 64 registers per thread at N = 128
+constexpr int T32_WIDE_MAX_N = 64;          // NWG = 4: 2 x 32 registers at N = 64 under the 96-register cap of 640 threads
+// warpgroup 0: producer + converters; warpgroups 1..NWG: consumers
+constexpr int t32_threads(int nwg) { return 128 * (nwg + 1); }
 constexpr int T32_STAGE_SLOTS = 2;          // fp32 staging boxes (TMA -> converters)
 constexpr int T32_PLANES = 2;               // operand planes: fp16(v), fp16(2^11 (v - fp16(v)))
 constexpr float T32_LO_SCALE = 2048.f, T32_LO_INV = 1.f / 2048.f;
@@ -47,7 +53,7 @@ constexpr float T32_LO_SCALE = 2048.f, T32_LO_INV = 1.f / 2048.f;
 __device__ unsigned int g_tc32_overflow = 0;     // activations / weights that exceeded the fp16 range of the main product
 
 struct Tc32Extra {
-  int rows;                  // activation rows (pixels) per A item: halo_h * halo_w, or 128
+  int rows;                  // activation rows (pixels) per A item: halo_h * halo_w, or the tile's 64 * NWG pixels
   int plane_bytes;           // bytes of one operand plane of an A item (rows * 64, padded to 1024)
   int stage_bytes;           // bytes of one fp32 staging slot (rows * 128, padded to 1024)
   int b_plane_bytes;         // block_n * 64: one weight plane of one step
@@ -378,28 +384,33 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
   }
 }
 
+template <int NWG>
 __device__ __forceinline__ void consumer32_n(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, int wg) {
   switch (p.block_n) {
     case 16: consumer32<16>(p, e, rg, wg); break;
     case 32: consumer32<32>(p, e, rg, wg); break;
     case 64: consumer32<64>(p, e, rg, wg); break;
-    default: consumer32<128>(p, e, rg, wg); break;
+    default:
+      if constexpr (NWG == 2) consumer32<T32_MAX_N>(p, e, rg, wg);
+      else __trap();                      // the host plan never pairs NWG = 4 with block_n > T32_WIDE_MAX_N
+      break;
   }
 }
 
 // barrier arrival counts: sfull / bfull = one TMA arrival, sempty = every converter thread, pfull = every converter thread
 // (convolution) or one arrival per 8-row sampling unit (DCN), pempty / bempty = one arrival per consumer warpgroup
-__device__ __forceinline__ void init_bars32(const Ring32& rg, uint32_t pfull_count, uint32_t sempty_count) {
+__device__ __forceinline__ void init_bars32(const Ring32& rg, uint32_t pfull_count, uint32_t sempty_count, uint32_t consumers) {
   for (int i = threadIdx.x & 31; i < T32_NBAR; i += 32) {
     const int kind = i / MAX_STAGES;       // 0 sfull, 1 sempty, 2 pfull, 3 pempty, 4 bfull, 5 bempty
-    const uint32_t count = kind == 1 ? sempty_count : (kind == 2 ? pfull_count : ((kind == 3 || kind == 5) ? 2u : 1u));
+    const uint32_t count = kind == 1 ? sempty_count : (kind == 2 ? pfull_count : ((kind == 3 || kind == 5) ? consumers : 1u));
     mbar_init(rg.bar_base + 8u * i, count);
   }
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- kernel
-__global__ void __launch_bounds__(T32_THREADS, 1)
+template <int NWG>
+__global__ void __launch_bounds__(t32_threads(NWG), 1)
 conv_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvTcParams p,
                        const Tc32Extra e) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -410,7 +421,7 @@ conv_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   rg.b_base = rg.a_base + (uint32_t)p.a_stages * rg.a_bytes; rg.b_bytes = (uint32_t)T32_PLANES * (uint32_t)e.b_plane_bytes;
   rg.bar_base = rg.b_base + (uint32_t)p.b_stages * rg.b_bytes;
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);     // warp-uniform role index (wgmma issue is not treated as divergent)
-  if (warp == 0) init_bars32(rg, 32 * T32_CONV_WARPS, 32 * T32_CONV_WARPS);
+  if (warp == 0) init_bars32(rg, 32 * T32_CONV_WARPS, 32 * T32_CONV_WARPS, NWG);
   if (threadIdx.x == 32) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
@@ -421,7 +432,7 @@ conv_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (warp == 0) producer32(p, e, rg, &tmA, &tmB);
   else if (warp < 4) converter32(p, e, rg, (int)threadIdx.x - 32, 32 * T32_CONV_WARPS);
-  else consumer32_n(p, e, rg, (warp - 4) >> 2);
+  else consumer32_n<NWG>(p, e, rg, (warp - 4) >> 2);
 }
 
 // ---------------------------------------------------------------- fused DCNv1 kernel (same pipeline, sampling warps feed the ring)
@@ -436,7 +447,7 @@ dcn_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmB, const ConvTcParam
   const uint32_t setup_base = rg.b_base + (uint32_t)p.b_stages * rg.b_bytes;
   rg.bar_base = setup_base + DCN32_SETUP_BYTES;
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);     // warp-uniform role index (wgmma issue is not treated as divergent)
-  if (warp == 0) init_bars32(rg, DCN32_UNITS_PER_STEP, 1);
+  if (warp == 0) init_bars32(rg, DCN32_UNITS_PER_STEP, 1, 2);
   if (threadIdx.x == 32) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
   __syncthreads();
   asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -501,6 +512,103 @@ inline int64_t plane_elems(int cout, int cin, int kh, int kw) {
   return cout_pad * kh * kw * cin_pad;
 }
 
+int num_sms32() {
+  if (!g_num_sms32) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&g_num_sms32, cudaDevAttrMultiProcessorCount, dev);
+  }
+  return g_num_sms32;
+}
+
+constexpr int T32_SMEM_BUDGET = 227 * 1024 - 1024 - T32_BAR_BYTES - 64;
+
+// Tiling of one tc32 launch.  Everything here follows from the shapes (and the SM count); vps_conv2d_tc32_multi launches
+// exactly this plan and vps_conv2d_tc32_plan reports it.
+struct Tc32Plan {
+  int nwg;                   // consumer warpgroups: the tile holds 64 * nwg output pixels
+  int block_n;
+  int halo, tw, th, halo_w, halo_h;
+  int rows, stage_bytes, plane_bytes, a_stages, a_side;    // A item rows, staging / operand-plane slot bytes, ring depth
+  int b_stages;
+};
+
+Tc32Plan tc32_tile(const vps_conv_args* a, int nwg) {
+  Tc32Plan g = {};
+  g.nwg = nwg;
+  const int px = 64 * nwg;
+  g.halo = a->sh == 1 && a->sw == 1 && a->kh * a->kw > 1 && a->kh <= 8 && a->kw <= 8;
+  if (g.halo) {          // 8-pixel halo rows: the consumer's descriptors step one halo row per 8-row group
+    g.tw = 8; g.th = px / 8;
+  } else {
+    int best_tw = 16; int64_t best_area = -1;
+    const int cands[6] = {16, 8, 32, 64, 128, 256};
+    for (int i = 0; i < 6; ++i) {
+      const int tw = cands[i], th = px / tw;
+      if (th == 0 || tw * a->sw > 256 || th * a->sh > 256) continue;     // TMA box extents
+      const int64_t area = (int64_t)vps::cdiv(a->ow, tw) * tw * vps::cdiv(a->oh, th) * th;
+      if (best_area < 0 || area < best_area) { best_area = area; best_tw = tw; }
+    }
+    g.tw = best_tw; g.th = px / best_tw;
+  }
+  g.halo_w = g.tw + a->kw - 1;
+  g.halo_h = g.th + a->kh - 1;
+  g.rows = g.halo ? g.halo_h * g.halo_w : px;
+  g.stage_bytes = (g.rows * 128 + 1023) / 1024 * 1024;
+  g.plane_bytes = (g.rows * 64 + 1023) / 1024 * 1024;
+  g.a_stages = g.halo ? 2 : 3;
+  g.a_side = T32_STAGE_SLOTS * g.stage_bytes + g.a_stages * T32_PLANES * g.plane_bytes;
+  return g;
+}
+
+// (NWG, block_n) minimising waves * (steps * step clocks + epilogue) over the candidates whose rings fit (>= 2 weight
+// stages).  block_n is a power-of-two divisor of cout_pad, <= 128 at NWG 2 and <= 64 at NWG 4 (the register cap).
+// A step of one warpgroup is two dependent wgmma round trips plus its barrier waits: ~300 clocks whatever N is (the latency
+// floor); its 6 MMAs take 3*bn clocks of the tensor pipe per 2 warpgroups, so 6*bn at NWG 4; its weight tile arrives at
+// the L2 rate (56 B/clk per SM); and the three converter warps turn an A item of `rows` pixels into operand planes at ~2
+// clocks per row -- in flat mode every step is a new item (256 rows at NWG 4), in halo mode one item feeds all taps.
+// So NWG 4 shares the latency floor among twice the pixels and halves the per-tile epilogue, and wins wherever the grid
+// has enough tiles; it loses where the converters bind: flat layers with many K steps whose cout_pad > 64 must be split
+// into more N tiles at NWG 4, each converting the same activations again (3x3 / stride 2, 128 -> 128 at 256x512 ran 15%
+// slower).  The 2 clocks per row is the value that keeps those on NWG 2 and every layer that measured faster on NWG 4;
+// per-layer H100 timings are in DESIGN.md §5.0.
+int tc32_plan(const vps_conv_args* a, int nprob, Tc32Plan& out) {
+  VPS_CHECK_ARG(nprob >= 1 && nprob <= MAX_PROB, "conv2d_tc32: nprob %d", nprob);
+  VPS_CHECK_ARG(a->sh >= 1 && a->sh <= 2 && a->sw >= 1 && a->sw <= 2, "conv2d_tc32: stride must be 1 or 2");
+  VPS_CHECK_ARG(a->kh >= 1 && a->kw >= 1 && a->cin >= 1 && a->cout >= 1 && a->oh >= 0 && a->ow >= 0 && a->x.n >= 0,
+                "conv2d_tc32: bad geometry (k %dx%d, cin %d, cout %d, out %dx%d)", a->kh, a->kw, a->cin, a->cout, a->oh, a->ow);
+  const int sms = num_sms32();
+  if (sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
+  const int cout_pad = (a->cout + 15) / 16 * 16;
+  const int steps = (a->cin + T32_KC - 1) / T32_KC * a->kh * a->kw;
+  double best = -1.0;
+  for (int nwg = 2; nwg <= 4; nwg += 2) {
+    Tc32Plan g = tc32_tile(a, nwg);
+    const int64_t m_tiles = (int64_t)a->x.n * vps::cdiv(a->oh, g.th) * vps::cdiv(a->ow, g.tw) * nprob;
+    const double conv = 2.0 * (g.halo ? (double)g.rows / (a->kh * a->kw) : (double)g.rows);
+    for (int bn = 16; bn <= (nwg == 2 ? T32_MAX_N : T32_WIDE_MAX_N) && bn <= cout_pad; bn *= 2) {
+      if (cout_pad % bn) continue;
+      if (g.a_side + 2 * bn * 64 * T32_PLANES > T32_SMEM_BUDGET) continue;
+      const int64_t tiles = m_tiles * (cout_pad / bn);
+      const double waves = (double)((tiles + sms - 1) / sms);
+      const double step = fmax(fmax(300.0, 1.5 * nwg * bn), fmax((double)(bn * 64 * T32_PLANES) / 56.0, conv));
+      const double t = waves * ((double)steps * step + 40.0 * bn + 1500.0);
+      if (best < 0 || t < best * 0.999) {
+        best = t;
+        out = g;
+        out.block_n = bn;
+      }
+    }
+  }
+  if (best < 0) {
+    vps::set_error("conv2d_tc32: ring does not fit (k %dx%d)", a->kh, a->kw);
+    return VPS_E_ARG;
+  }
+  const int bst = (T32_SMEM_BUDGET - out.a_side) / (T32_PLANES * out.block_n * 64);
+  out.b_stages = bst > MAX_STAGES ? MAX_STAGES : bst;
+  return VPS_OK;
+}
+
 }  // namespace
 
 extern "C" int64_t vps_packed_tc32_bytes(int cout, int cin, int kh, int kw, int nprob) {
@@ -547,7 +655,6 @@ extern "C" int vps_conv2d_tc32_multi(const vps_conv_args* args, int nprob, void*
   const vps_conv_args* a = &args[0];
   VPS_CHECK_ARG(a->x.dtype == VPS_F32, "conv2d_tc32: x must be fp32");
   VPS_CHECK_ARG(a->x.cs % 4 == 0 && ((uintptr_t)a->x.ptr & 15) == 0, "conv2d_tc32: x not 16B aligned (cs=%d)", a->x.cs);
-  VPS_CHECK_ARG(a->sh >= 1 && a->sh <= 2 && a->sw >= 1 && a->sw <= 2, "conv2d_tc32: stride must be 1 or 2");
   VPS_CHECK_ARG(a->cin == a->x.c, "conv2d_tc32: cin %d != x.c %d", a->cin, a->x.c);
   VPS_CHECK_ARG(((uintptr_t)a->w & 127) == 0, "conv2d_tc32: weights not aligned");
   for (int i = 0; i < nprob; ++i) {
@@ -558,39 +665,25 @@ extern "C" int vps_conv2d_tc32_multi(const vps_conv_args* args, int nprob, void*
   }
   auto encode = get_encode32();
   if (!encode) { vps::set_error("cuTensorMapEncodeTiled unavailable"); return VPS_E_CUDA; }
-  if (!g_num_sms32) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms32, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms32 <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
-  }
+  Tc32Plan g;
+  const int st = tc32_plan(a, nprob, g);
+  if (st != VPS_OK) return st;
+  VPS_CHECK_ARG(g.b_stages >= 2, "conv2d_tc32: ring does not fit (%d x %d px halo, bn %d)", g.halo_h, g.halo_w, g.block_n);
   ConvTcParams p = {};
   Tc32Extra e = {};
   p.bk = T32_KC;
   const int cin_pad = (a->cin + T32_KC - 1) / T32_KC * T32_KC;
   const int cout_pad = (a->cout + 15) / 16 * 16;
   p.n_img = a->x.n; p.oh = a->oh; p.ow = a->ow;
-  const bool halo = a->sh == 1 && a->sw == 1 && a->kh * a->kw > 1 && a->kh <= 8 && a->kw <= 8;
-  p.halo = halo ? 1 : 0;
-  if (halo) {
-    p.tw = 8; p.th = 16;
-  } else {
-    int best_tw = 16; int64_t best_area = -1;
-    const int cands[5] = {16, 8, 32, 64, 128};
-    for (int i = 0; i < 5; ++i) {
-      const int tw = cands[i], th = 128 / tw;
-      if (tw * a->sw > 256 || th * a->sh > 256) continue;
-      const int64_t area = (int64_t)vps::cdiv(a->ow, tw) * tw * vps::cdiv(a->oh, th) * th;
-      if (best_area < 0 || area < best_area) { best_area = area; best_tw = tw; }
-    }
-    p.tw = best_tw; p.th = 128 / best_tw;
-  }
-  p.halo_w = p.tw + a->kw - 1;
-  const int halo_h = p.th + a->kh - 1;
-  e.rows = halo ? halo_h * p.halo_w : BLOCK_M;
+  const bool halo = g.halo != 0;
+  p.halo = g.halo;
+  p.tw = g.tw; p.th = g.th;
+  p.halo_w = g.halo_w;
+  const int halo_h = g.halo_h;
+  e.rows = g.rows;
   p.a_box_bytes = e.rows * 128;
-  e.stage_bytes = (e.rows * 128 + 1023) / 1024 * 1024;
-  e.plane_bytes = (e.rows * 64 + 1023) / 1024 * 1024;
+  e.stage_bytes = g.stage_bytes;
+  e.plane_bytes = g.plane_bytes;
   p.a_stage_bytes = T32_PLANES * e.plane_bytes;
   p.tiles_x = vps::cdiv(a->ow, p.tw); p.tiles_y = vps::cdiv(a->oh, p.th);
   p.kh = a->kh; p.kw = a->kw; p.sh = a->sh; p.sw = a->sw;
@@ -598,33 +691,11 @@ extern "C" int vps_conv2d_tc32_multi(const vps_conv_args* args, int nprob, void*
   const int rem = a->cin - (p.cin_chunks - 1) * T32_KC;
   e.nk_last = (rem + 15) / 16;
   const int ntaps = a->kh * a->kw;
-  p.a_stages = halo ? 2 : 3;
-  const int smem_budget = 227 * 1024 - 1024 - T32_BAR_BYTES - 64;
-  const int a_side = T32_STAGE_SLOTS * e.stage_bytes + p.a_stages * p.a_stage_bytes;
-  // N tile: a power-of-two divisor of cout_pad (16 .. 128, the extents the consumer is instantiated for) minimising
-  // waves * (steps * step clocks + epilogue); a step is 6 MMAs = 3*bn clocks at the MMA floor, ~300 clocks of issue /
-  // barrier latency, or its weight bytes at the L2 rate
-  int block_n = 16;
-  {
-    const int64_t m_tiles = (int64_t)a->x.n * p.tiles_y * p.tiles_x * nprob;
-    double best = -1.0;
-    for (int bn = 16; bn <= T32_MAX_N && bn <= cout_pad; bn *= 2) {
-      if (cout_pad % bn) continue;
-      if (a_side + 2 * bn * 64 * T32_PLANES > smem_budget) continue;
-      const int64_t tiles = m_tiles * (cout_pad / bn);
-      const double waves = (double)((tiles + g_num_sms32 - 1) / g_num_sms32);
-      const double step = fmax(fmax(300.0, 3.0 * bn), (double)(bn * 64 * T32_PLANES) / 56.0);
-      const double t = waves * ((double)(p.cin_chunks * ntaps) * step + 40.0 * bn + 1500.0);
-      if (best < 0 || t < best * 0.999) { best = t; block_n = bn; }
-    }
-  }
+  p.a_stages = g.a_stages;
+  const int block_n = g.block_n;
   p.block_n = block_n; p.n_tiles_n = cout_pad / block_n;
   e.b_plane_bytes = block_n * 64;
-  {
-    int bst = (smem_budget - a_side) / (T32_PLANES * e.b_plane_bytes);
-    p.b_stages = bst > MAX_STAGES ? MAX_STAGES : bst;
-    VPS_CHECK_ARG(p.b_stages >= 2, "conv2d_tc32: ring does not fit (%d x %d px halo, bn %d)", halo_h, p.halo_w, block_n);
-  }
+  p.b_stages = g.b_stages;
   { static int sl_env = -1; if (sl_env < 0) { const char* ev = getenv("VPS_TC32_SLEEP"); sl_env = ev ? atoi(ev) : 0; } e.sleep_ns = sl_env; }
   p.nprob = nprob;
   p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
@@ -673,32 +744,41 @@ extern "C" int vps_conv2d_tc32_multi(const vps_conv_args* args, int nprob, void*
                         CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { vps::set_error("conv2d_tc32: encode B failed (%d)", (int)r); return VPS_E_CUDA; }
   }
-  const int smem = a_side + p.b_stages * T32_PLANES * e.b_plane_bytes + 1024 + T32_BAR_BYTES;
-  static bool smem_set = false;
-  if (!smem_set) {
-    if (cudaFuncSetAttribute(conv_igemm_tc32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
+  const int smem = g.a_side + p.b_stages * T32_PLANES * e.b_plane_bytes + 1024 + T32_BAR_BYTES;
+  const auto kernel = g.nwg == 4 ? conv_igemm_tc32_kernel<4> : conv_igemm_tc32_kernel<2>;
+  static bool smem_set[2] = {false, false};
+  if (!smem_set[g.nwg == 4]) {
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
       vps::set_error("conv2d_tc32: cannot raise dynamic smem: %s", cudaGetErrorString(cudaGetLastError()));
       return VPS_E_CUDA;
     }
-    smem_set = true;
+    smem_set[g.nwg == 4] = true;
   }
   const int grid = p.total_tiles < g_num_sms32 ? p.total_tiles : g_num_sms32;
   static int pdl_env = -1;
   if (pdl_env < 0) { const char* ev = getenv("VPS_PDL"); pdl_env = ev ? atoi(ev) : 1; }
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(T32_THREADS); cfg.dynamicSmemBytes = (size_t)smem;
+  cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(t32_threads(g.nwg)); cfg.dynamicSmemBytes = (size_t)smem;
   cfg.stream = (cudaStream_t)stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = pdl_env ? 1 : 0;
-  const cudaError_t le = cudaLaunchKernelEx(&cfg, conv_igemm_tc32_kernel, tmA, tmB, p, e);
+  const cudaError_t le = cudaLaunchKernelEx(&cfg, kernel, tmA, tmB, p, e);
   if (le != cudaSuccess) { vps::set_error("conv2d_tc32: launch failed: %s", cudaGetErrorString(le)); return VPS_E_CUDA; }
   VPS_CUDA_LAST("conv_igemm_tc32_kernel");
   return VPS_OK;
 }
 
 extern "C" int vps_conv2d_tc32(const vps_conv_args* a, void* stream) { return vps_conv2d_tc32_multi(a, 1, stream); }
+
+extern "C" int vps_conv2d_tc32_plan(const vps_conv_args* a, int nprob, int* plan) {
+  Tc32Plan g;
+  const int st = tc32_plan(a, nprob, g);
+  if (st != VPS_OK) return st;
+  plan[0] = g.nwg; plan[1] = g.block_n; plan[2] = g.tw; plan[3] = g.th; plan[4] = g.halo;
+  return VPS_OK;
+}
 
 
 // Fused DCNv1 3x3 / stride 1 / pad 1 / dilation 1 / 1 deformable group in the tc32 precision (deform_conv.py:15-87 forward,
@@ -715,12 +795,7 @@ extern "C" int vps_deform_conv_tc32(const vps_tensor* x, const vps_tensor* offse
   VPS_CHECK_ARG(((uintptr_t)w & 127) == 0, "deform_conv_tc32: weights not aligned");
   auto encode = get_encode32();
   if (!encode) { vps::set_error("cuTensorMapEncodeTiled unavailable"); return VPS_E_CUDA; }
-  if (!g_num_sms32) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms32, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms32 <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
-  }
+  if (num_sms32() <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
   const int cout_pad = (cout + 15) / 16 * 16;
   ConvTcParams p = {};
   Tc32Extra e = {};

@@ -268,6 +268,20 @@ def conv2d_tc_multi(x, pws, y, pads, omaps, act=ACT_NONE, slope=0.1, out_scale=1
     return y
 
 
+def conv2d_tc32_plan(x, pws, stride=1, pad=0, oh=None, ow=None, pads=None):
+    """The tiling the tc32 kernel picks for conv2d (one problem) or conv2d_tc_multi (`pads` = per-phase (ph, pw), stride 1):
+    dict(nwg=consumer warpgroups (2 or 4), block_n, tw, th (output pixels per tile), halo)."""
+    pws = pws if isinstance(pws, (list, tuple)) else [pws]
+    n = len(pws)
+    arr = (VpsConvArgs * n)()
+    for i in range(n):
+        arr[i] = _conv_args(x, pws[i], x, stride, pad, ACT_NONE, 0.1, None, False, 1.0, oh, ow, (1, 0, 1, 0),
+                            pads[i] if pads is not None else None)
+    plan = (C.c_int * 5)()
+    check(_real_lib().vps_conv2d_tc32_plan(arr, n, plan), "conv2d_tc32_plan")
+    return dict(nwg=plan[0], block_n=plan[1], tw=plan[2], th=plan[3], halo=plan[4])
+
+
 # ------------------------------------------------------------------ FlowNet2 native ops
 def correlation(f1, f2, out, pad, max_disp, stride1, stride2, act=ACT_NONE, slope=0.1, impl=None):
     """impl: None = dispatch (tensor cores for bf16 features, and for fp32 features in the tc32 precision), "tc" / "tc32" /
