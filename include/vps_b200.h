@@ -116,7 +116,9 @@ int vps_conv2d_tc32_multi(const vps_conv_args* a, int nprob, void* stream);
 /* The tiling vps_conv2d_tc32_multi(a, nprob) launches, from the shapes in `a` and the current device's SM count (no
  * pointer is read): plan[0] = consumer warpgroups (2: 128-pixel tiles, block_n <= 128; 4: 256-pixel tiles, block_n <= 64),
  * plan[1] = block_n, plan[2] = tile width, plan[3] = tile height (output pixels), plan[4] = 1 in halo mode (stride 1,
- * > 1 tap: one activation box per 32-channel chunk feeds every tap). */
+ * > 1 tap: one activation box per 32-channel chunk feeds every tap), plan[5] = 1 for the TMA epilogue (results staged in
+ * shared memory and stored by TMA; one fp32 problem with 16-byte aligned output / residual slices, block_n <= 64, and
+ * room in shared memory), 0 for stores straight from the accumulator fragments.  `plan` holds 6 ints. */
 int vps_conv2d_tc32_plan(const vps_conv_args* a, int nprob, int* plan);
 int vps_pack_weights_tc32(const float* w_oihw, const float* scale, void* dst, int cout, int cin, int kh, int kw,
                           int transposed, int prob, int nprob, void* stream);

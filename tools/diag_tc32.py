@@ -87,13 +87,14 @@ def main():
             r.copy_(torch.randn(n, oh, ow, cout, generator=g).to(dev))
         pad = k // 2 if s == 1 or k % 2 else 1
         f = lambda: ops.conv2d(x, pk, y, stride=s, pad=pad, act=ops.ACT_RELU, res=r, use_tc=True, oh=oh, ow=ow)
+        plan = ops.conv2d_tc32_plan(x, pk, stride=s, pad=pad, oh=oh, ow=ow, y=y, res=r)
         sys.stderr.flush()
         ms = timeit(f, iters)
         fl = 2.0 * n * oh * ow * cout * cin * k * k
         by = 4.0 * n * (h * w * cin + oh * ow * cout * (2 if res else 1))
-        print("%-28s %dx%d s%d %4d->%4d @%dx%d n%d: %.4f ms  %6.1f TF/s alg  %6.1f MB  hbm-floor %.4f ms (%.2f of it)" %
-              (note, k, k, s, cin, cout, oh, ow, n, ms, fl / ms / 1e9, by / 1e6, by / HBM_GBPS / 1e6, by / HBM_GBPS / 1e6 / ms),
-              flush=True)
+        print("%-28s %dx%d s%d %4d->%4d @%dx%d n%d: %.4f ms  %6.1f TF/s alg  %6.1f MB  hbm-floor %.4f ms (%.2f of it)  "
+              "nwg %d bn %d %s" % (note, k, k, s, cin, cout, oh, ow, n, ms, fl / ms / 1e9, by / 1e6, by / HBM_GBPS / 1e6,
+                                   by / HBM_GBPS / 1e6 / ms, plan["nwg"], plan["block_n"], plan["epilogue"]), flush=True)
         del x, y, r, pk
     from vps_b200.layers import deconv4x4_s2
     for (n, cin, cout, h, w, note) in DECONVS:

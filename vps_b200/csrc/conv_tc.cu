@@ -232,7 +232,7 @@ __device__ __forceinline__ void consumer_tc(const ConvTcParams& p, const Ring& r
     wg::wait<0>();
     wg::fence_regs(d);
     rel.flush(rg, leader);
-    epi_frag<N>(p, d, tile, wg * 64);
+    epi_frag<N, 2>(p, d, tile, wg * 64);
   }
 }
 

@@ -29,7 +29,10 @@
 //                     fence.proxy.async -> mbarrier).  In halo mode (stride 1, > 1 tap) one converted (th+kh-1) x (tw+kw-1)
 //                     box feeds all kh*kw taps through shifted descriptor start addresses.
 //   warpgroups 1..NWG: consumers, pixels 64 wg .. 64 wg + 63: wgmma.kind f16 (M64 x N x K16) into registers, promotion, then
-//                     bias / activation / residual and the NHWC store straight from the accumulator fragments.
+//                     bias / activation / residual and the NHWC store.  Flat tiles (block_n <= 64, aligned fp32 output)
+//                     stage the result in shared-memory output boxes and store them by TMA while the next tile's K steps
+//                     run, the residual having arrived by TMA during the K steps; halo tiles and outputs no tensor map
+//                     expresses store straight from the accumulator fragments.
 // NWG = 2 (384 threads, block_n <= 128) or 4 (640 threads, block_n <= 64).  A K step is two dependent wgmma round trips
 // (the promotion order above), so a warpgroup spends a fixed few hundred clocks per step whatever N is; at N <= 64 four
 // warpgroups overlap those round trips and share each converted box and weight tile among twice the pixels.  At 640
@@ -80,6 +83,7 @@ struct Ring32 {
   uint32_t s_base, s_bytes;      // staging ring
   uint32_t a_base, a_bytes;      // operand-plane ring (T32_PLANES planes per slot)
   uint32_t b_base, b_bytes;      // weight ring (T32_PLANES planes per slot)
+  uint32_t e_base, bias_base;    // TMA epilogue: the consumers' output boxes, their block_n bias values
   uint32_t bar_base;
   __device__ __forceinline__ uint32_t sfull(int s) const { return bar_base + 8u * s; }
   __device__ __forceinline__ uint32_t sempty(int s) const { return bar_base + 8u * (MAX_STAGES + s); }
@@ -88,9 +92,17 @@ struct Ring32 {
   __device__ __forceinline__ uint32_t bfull(int s) const { return bar_base + 8u * (4 * MAX_STAGES + s); }
   __device__ __forceinline__ uint32_t bempty(int s) const { return bar_base + 8u * (5 * MAX_STAGES + s); }
   __device__ __forceinline__ uint32_t unit_ctr() const { return bar_base + 8u * (6 * MAX_STAGES); }   // DCN sampling units
+  __device__ __forceinline__ uint32_t rfull(int wg) const { return bar_base + 8u * (6 * MAX_STAGES + 1 + wg); }  // residual box
 };
 constexpr int T32_NBAR = 6 * MAX_STAGES;
-constexpr int T32_BAR_BYTES = 8 * (T32_NBAR + 2);
+constexpr int T32_BAR_BYTES = 8 * (T32_NBAR + 2 + 4);
+// TMA epilogue: a warpgroup's 64 x N result is stored as N / t32_box_c(N) boxes of t32_box_c(N) channels (128- or 64-byte
+// rows, SWIZZLE_128B / SWIZZLE_64B) x 64 pixels (min(tw, 64) wide)
+constexpr int t32_box_c(int n) { return n >= 32 ? 32 : 16; }
+// At N = 128 the sum alone takes 64 of the 168 registers of a 384-thread CTA, and the TMA epilogue's unrolled pass over it
+// spills around the slow-path call of the sigmoid's IEEE division; those tiles keep the fragment epilogue.
+constexpr int T32_EPI_MAX_N = 64;
+constexpr int t32_epi_bytes(int nwg, int bn) { return 64 * nwg * bn * 4 + nwg * bn * 4; }    // output boxes + bias
 
 __device__ __forceinline__ void tma_load_5d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, int c3,
                                             int c4) {
@@ -99,6 +111,12 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const void* tmap, uint
       "%4, %5, %6, %7}], [%2];" ::"r"(dst),
       "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
+}
+// shared -> global tensor store of one box (clipped at the tensor bounds), in the issuing thread's bulk async-group
+__device__ __forceinline__ void tma_store_4d(const void* tmap, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(tmap), "r"(src),
+               "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
 }
 // fp16 (round to nearest, saturating) of v; `over` collects |v| > 65504 (and NaN)
 __device__ __forceinline__ float to_f16_sat(float v, unsigned short& bits, bool& over) {
@@ -319,12 +337,83 @@ __device__ __forceinline__ void dcn_gather32(const ConvTcParams& p, const Tc32Ex
   }
 }
 
+// ---------------------------------------------------------------- TMA epilogue
+// Byte address of (pixel q of the warpgroup, tile channel c) in the warpgroup's output boxes, swizzled as TMA reads and writes
+// them: 16-byte chunk k of pixel row q sits at k ^ (q & 7) (SWIZZLE_128B, 32-channel rows) or k ^ ((q >> 1) & 3)
+// (SWIZZLE_64B, 16-channel rows).  The float2 stores of a warp then cover every bank twice: two wavefronts, no conflict.
+template <int N>
+__device__ __forceinline__ uint32_t epi_box_addr(uint32_t box, int q, int c) {
+  constexpr int BC = t32_box_c(N);
+  const uint32_t k = (uint32_t)((c % BC) >> 2);
+  const uint32_t sw = BC == 32 ? (uint32_t)(q & 7) : (uint32_t)((q >> 1) & 3);
+  return box + (uint32_t)(c / BC) * (64u * BC * 4u) + (uint32_t)q * (BC * 4u) + ((k ^ sw) << 4) + (uint32_t)(c & 3) * 4u;
+}
+
+// The output box of warpgroup wg in tile `tile`: channels n0.., pixels (x0, y0).. of image img; live = any pixel in range.
+// Recomputed where it is needed rather than held in registers across the K steps.
+struct EpiBox {
+  int n0, x0, y0, img;
+  bool live;
+};
+__device__ __forceinline__ EpiBox epi_box(const ConvTcParams& p, int tile, int wg) {
+  const TileCoord t = tile_coord(p, tile);
+  EpiBox b;
+  b.n0 = t.n_idx * p.block_n; b.img = t.img;
+  b.x0 = t.tx * p.tw + (64 * wg) % p.tw; b.y0 = t.ty * p.th + (64 * wg) / p.tw;
+  b.live = b.x0 < p.ow && b.y0 < p.oh;
+  return b;
+}
+
+// One warpgroup's 64 x N result -> its output boxes (residual read from, and the result written over, the box the TMA load
+// filled) -> TMA store of the boxes.  The store stays in flight while the warpgroup runs the next tile's K steps.  The
+// boxes are written again only after the leader's cp.async.bulk.wait_group.read, i.e. once the store has read them.
+template <int N>
+__device__ __forceinline__ void epi_tma32(const ConvTcParams& p, const CUtensorMap* tmY, const float (&d)[N / 2], uint32_t box,
+                                          uint32_t bias_s, float bias_v, uint32_t rbar, uint32_t rphase, int wg, int tile) {
+  constexpr int BC = t32_box_c(N);
+  const int i = threadIdx.x & 127, lane = threadIdx.x & 31, w = i >> 5;
+  if (i < N) asm volatile("st.shared.f32 [%0], %1;" ::"r"(bias_s + 4u * i), "f"(bias_v) : "memory");
+  if (i == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+  asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");        // bias visible, boxes free
+  if (p.res) mbar_wait(rbar, rphase);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int q = 16 * w + (lane >> 2) + 8 * h;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      const int c = 8 * j + 2 * (lane & 3);
+      const uint32_t a = epi_box_addr<N>(box, q, c);
+      float b0, b1, r0 = 0.f, r1 = 0.f;
+      asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(b0), "=f"(b1) : "r"(bias_s + 4u * c));
+      if (p.res) asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(r0), "=f"(r1) : "r"(a));
+      const float2 v = epi_math(p, d[4 * j + 2 * h], d[4 * j + 2 * h + 1], b0, b1, r0, r1);
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(v.x), "f"(v.y) : "memory");
+    }
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");        // generic-proxy writes -> TMA reads
+  asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+  const EpiBox eb = epi_box(p, tile, wg);
+  if (i == 0 && eb.live) {
+#pragma unroll
+    for (int b = 0; b < N / BC; ++b) tma_store_4d(tmY, box + (uint32_t)b * (64u * BC * 4u), eb.n0 + b * BC, eb.x0, eb.y0, eb.img);
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+  }
+}
+
 // ---------------------------------------------------------------- consumer warpgroups: MMA, promotion, epilogue
 // Per K step: acc = A2*B + A*B2 (fresh chain), acc *= 2^-11, acc += A*B, sum += acc (round to nearest).  The operand planes
 // and weight tiles of the step are released as soon as its MMAs have completed (one arrival per consumer warpgroup).
-template <int N>
-__device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, int wg) {
+// With the TMA epilogue the leader loads the tile's residual boxes after the first K step: by then the previous tile's store
+// has long read the boxes, so its wait does not hold up the first MMAs.
+template <int N, bool TMA_EPI>
+__device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, int wg,
+                                           const CUtensorMap* tmY, const CUtensorMap* tmR) {
+  constexpr int BC = t32_box_c(N);
   const bool leader = (threadIdx.x & 127) == 0;
+  constexpr bool epi_tma = TMA_EPI;
+  const uint32_t box = rg.e_base + (uint32_t)wg * (64u * N * 4u), bias_s = rg.bias_base + (uint32_t)wg * (N * 4u);
+  const uint32_t rbar = rg.rfull(wg);
+  uint32_t rphase = 0;
   const bool halo = p.halo != 0;
   const int ntaps = p.kh * p.kw, kw = p.kw, last_cc = p.cin_chunks - 1;
   const uint32_t a_pitch = halo ? (uint32_t)p.halo_w * 64u : 512u;      // byte distance of the A planes' 8-row groups
@@ -336,6 +425,11 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
   int as = 0, bs = 0;
   uint32_t aphase = 0, bphase = 0;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    float bias_v = 0.f;
+    if (epi_tma) {        // this thread's bias value of the tile: loaded now, written to shared memory in the epilogue
+      const int c = tile_coord(p, tile).n_idx * N + (threadIdx.x & 127);
+      if (p.bias && (threadIdx.x & 127) < N && c < p.cout) bias_v = __ldg(p.bias + c);
+    }
 #pragma unroll
     for (int i = 0; i < N / 2; ++i) sum[i] = 0.f;
     for (int cc = 0; cc <= last_cc; ++cc) {
@@ -374,25 +468,46 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
         if (leader) {
           mbar_arrive(rg.bempty(bs));
           if (item_done) mbar_arrive(rg.pempty(as));
+          if (epi_tma && p.res && cc == 0 && tap == 0) {
+            asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+            const EpiBox eb = epi_box(p, tile, wg);
+            if (eb.live) {
+              mbar_expect_tx(rbar, 64u * N * 4u);
+#pragma unroll
+              for (int b = 0; b < N / BC; ++b)
+                tma_load_4d(box + (uint32_t)b * (64u * BC * 4u), tmR, rbar, eb.n0 + b * BC, eb.x0, eb.y0, eb.img);
+            } else {
+              mbar_arrive(rbar);
+            }
+          }
         }
         if (item_done && ++as == p.a_stages) { as = 0; aphase ^= 1; }
         if (++bs == p.b_stages) { bs = 0; bphase ^= 1; }
         if (++s == kw) { s = 0; ++r; }
       }
     }
-    epi_frag<N>(p, sum, tile, wg * 64);
+    if (epi_tma) {
+      epi_tma32<N>(p, tmY, sum, box, bias_s, bias_v, rbar, rphase, wg, tile);
+      if (p.res) rphase ^= 1u;
+    } else {
+      epi_frag<N, 4>(p, sum, tile, wg * 64);
+    }
   }
+  // the boxes must stay allocated until the last store has read them, and the stores must be complete before the grid is
+  // (a dependent launch's griddepcontrol.wait reads the output)
+  if (epi_tma && leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
-template <int NWG>
-__device__ __forceinline__ void consumer32_n(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, int wg) {
+template <int NWG, bool TMA_EPI>
+__device__ __forceinline__ void consumer32_n(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, int wg,
+                                             const CUtensorMap* tmY, const CUtensorMap* tmR) {
   switch (p.block_n) {
-    case 16: consumer32<16>(p, e, rg, wg); break;
-    case 32: consumer32<32>(p, e, rg, wg); break;
-    case 64: consumer32<64>(p, e, rg, wg); break;
+    case 16: consumer32<16, TMA_EPI>(p, e, rg, wg, tmY, tmR); break;
+    case 32: consumer32<32, TMA_EPI>(p, e, rg, wg, tmY, tmR); break;
+    case 64: consumer32<64, TMA_EPI>(p, e, rg, wg, tmY, tmR); break;
     default:
-      if constexpr (NWG == 2) consumer32<T32_MAX_N>(p, e, rg, wg);
-      else __trap();                      // the host plan never pairs NWG = 4 with block_n > T32_WIDE_MAX_N
+      if constexpr (NWG == 2 && !TMA_EPI) consumer32<T32_MAX_N, false>(p, e, rg, wg, tmY, tmR);
+      else __trap();                      // the host plan pairs block_n > T32_EPI_MAX_N with neither NWG = 4 nor the TMA epilogue
       break;
   }
 }
@@ -405,13 +520,15 @@ __device__ __forceinline__ void init_bars32(const Ring32& rg, uint32_t pfull_cou
     const uint32_t count = kind == 1 ? sempty_count : (kind == 2 ? pfull_count : ((kind == 3 || kind == 5) ? consumers : 1u));
     mbar_init(rg.bar_base + 8u * i, count);
   }
+  if ((threadIdx.x & 31) < 4) mbar_init(rg.rfull(threadIdx.x & 31), 1u);     // residual boxes: one TMA arrival
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- kernel
-template <int NWG>
+template <int NWG, bool TMA_EPI>
 __global__ void __launch_bounds__(t32_threads(NWG), 1)
-conv_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvTcParams p,
+conv_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmR, const ConvTcParams p,
                        const Tc32Extra e) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -419,12 +536,18 @@ conv_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   rg.s_base = smem_base; rg.s_bytes = (uint32_t)e.stage_bytes;
   rg.a_base = rg.s_base + T32_STAGE_SLOTS * rg.s_bytes; rg.a_bytes = (uint32_t)T32_PLANES * (uint32_t)e.plane_bytes;
   rg.b_base = rg.a_base + (uint32_t)p.a_stages * rg.a_bytes; rg.b_bytes = (uint32_t)T32_PLANES * (uint32_t)e.b_plane_bytes;
-  rg.bar_base = rg.b_base + (uint32_t)p.b_stages * rg.b_bytes;
+  rg.e_base = rg.b_base + (uint32_t)p.b_stages * rg.b_bytes;          // 1024-aligned: the ring slots are multiples of 1 KB
+  rg.bias_base = rg.e_base + (TMA_EPI ? 64u * NWG * (uint32_t)p.block_n * 4u : 0u);
+  rg.bar_base = rg.bias_base + (TMA_EPI ? (uint32_t)NWG * (uint32_t)p.block_n * 4u : 0u);
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);     // warp-uniform role index (wgmma issue is not treated as divergent)
   if (warp == 0) init_bars32(rg, 32 * T32_CONV_WARPS, 32 * T32_CONV_WARPS, NWG);
   if (threadIdx.x == 32) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+    if (TMA_EPI) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmY) : "memory");
+      if (p.res) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmR) : "memory");
+    }
   }
   __syncthreads();
   // programmatic dependent launch: the prologue above overlaps the previous kernel's tail (see conv_tc.cu)
@@ -432,7 +555,7 @@ conv_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (warp == 0) producer32(p, e, rg, &tmA, &tmB);
   else if (warp < 4) converter32(p, e, rg, (int)threadIdx.x - 32, 32 * T32_CONV_WARPS);
-  else consumer32_n<NWG>(p, e, rg, (warp - 4) >> 2);
+  else consumer32_n<NWG, TMA_EPI>(p, e, rg, (warp - 4) >> 2, &tmY, &tmR);
 }
 
 // ---------------------------------------------------------------- fused DCNv1 kernel (same pipeline, sampling warps feed the ring)
@@ -454,9 +577,9 @@ dcn_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmB, const ConvTcParam
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (warp >= 4 && warp < 12) {
     const int wg = (warp - 4) >> 2;
-    if (p.block_n == 16) consumer32<16>(p, e, rg, wg);
-    else if (p.block_n == 32) consumer32<32>(p, e, rg, wg);
-    else consumer32<DCN32_MAX_N>(p, e, rg, wg);
+    if (p.block_n == 16) consumer32<16, false>(p, e, rg, wg, nullptr, nullptr);
+    else if (p.block_n == 32) consumer32<32, false>(p, e, rg, wg, nullptr, nullptr);
+    else consumer32<DCN32_MAX_N, false>(p, e, rg, wg, nullptr, nullptr);
   } else if (warp == 0) {
     producer32(p, e, rg, &tmB, &tmB);
   } else {
@@ -531,7 +654,20 @@ struct Tc32Plan {
   int halo, tw, th, halo_w, halo_h;
   int rows, stage_bytes, plane_bytes, a_stages, a_side;    // A item rows, staging / operand-plane slot bytes, ring depth
   int b_stages;
+  int epi_tma;               // 1: TMA epilogue (output boxes in shared memory), 0: stores from the accumulator fragments
 };
+
+// A tensor map can express the output (and the residual) of one problem written at unit output strides into fp32 tensors
+// whose channel-slice base and pixel stride are 16-byte aligned.  The stride phases of a transposed convolution (nprob > 1,
+// doubled output strides), bf16 outputs or residuals and unaligned slices keep the fragment epilogue.
+bool tc32_epi_expressible(const vps_conv_args* a, int nprob) {
+  if (nprob != 1 || a->oy_mul != 1 || a->ox_mul != 1 || a->y.dtype != VPS_F32) return false;
+  const int64_t px = (int64_t)a->oy_off * a->y.w + a->ox_off;       // the first output pixel
+  if ((((uintptr_t)a->y.ptr + px * a->y.cs * 4) & 15) || a->y.cs % 4) return false;
+  if (a->res.ptr && (a->res.dtype != VPS_F32 || (((uintptr_t)a->res.ptr + px * a->res.cs * 4) & 15) || a->res.cs % 4))
+    return false;
+  return true;
+}
 
 Tc32Plan tc32_tile(const vps_conv_args* a, int nwg) {
   Tc32Plan g = {};
@@ -604,7 +740,22 @@ int tc32_plan(const vps_conv_args* a, int nprob, Tc32Plan& out) {
     vps::set_error("conv2d_tc32: ring does not fit (k %dx%d)", a->kh, a->kw);
     return VPS_E_ARG;
   }
-  const int bst = (T32_SMEM_BUDGET - out.a_side) / (T32_PLANES * out.block_n * 64);
+  // Epilogue: the TMA epilogue on flat tiles (one A item per K step: 1x1 and strided layers, a few K steps per tile, so the
+  // exposed epilogue was up to half of the layer) where it is expressible and its output boxes fit next to >= 2 weight
+  // stages, giving up the third operand-plane slot if need be (NWG 4 at block_n 64: 256-pixel A items).  Halo tiles keep the
+  // fragment epilogue: they run tens of K steps per tile, and the boxes would take the weight stages their taps stream
+  // through (NWG 4 at block_n 32 drops from 6 to 2 and ran 13-16% slower; per-layer H100 timings in DESIGN.md §5.0).
+  const int eb = t32_epi_bytes(out.nwg, out.block_n), b2 = 2 * T32_PLANES * out.block_n * 64;
+  out.epi_tma = 0;
+  if (!out.halo && out.block_n <= T32_EPI_MAX_N && tc32_epi_expressible(a, nprob)) {
+    if (out.a_side + b2 + eb > T32_SMEM_BUDGET && out.a_stages == 3 &&
+        out.a_side - T32_PLANES * out.plane_bytes + b2 + eb <= T32_SMEM_BUDGET) {
+      out.a_stages = 2;
+      out.a_side -= T32_PLANES * out.plane_bytes;
+    }
+    out.epi_tma = out.a_side + b2 + eb <= T32_SMEM_BUDGET;
+  }
+  const int bst = (T32_SMEM_BUDGET - out.a_side - (out.epi_tma ? eb : 0)) / (T32_PLANES * out.block_n * 64);
   out.b_stages = bst > MAX_STAGES ? MAX_STAGES : bst;
   return VPS_OK;
 }
@@ -744,15 +895,36 @@ extern "C" int vps_conv2d_tc32_multi(const vps_conv_args* args, int nprob, void*
                         CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { vps::set_error("conv2d_tc32: encode B failed (%d)", (int)r); return VPS_E_CUDA; }
   }
-  const int smem = g.a_side + p.b_stages * T32_PLANES * e.b_plane_bytes + 1024 + T32_BAR_BYTES;
-  const auto kernel = g.nwg == 4 ? conv_igemm_tc32_kernel<4> : conv_igemm_tc32_kernel<2>;
-  static bool smem_set[2] = {false, false};
-  if (!smem_set[g.nwg == 4]) {
+  // TMA epilogue: output and residual as [n][oh][ow][cout] from the first output pixel (a channel slice of a wider tensor
+  // keeps its pixel stride); TMA clips the boxes at oh / ow / cout, so partial tiles and the neighbouring channels are safe
+  CUtensorMap tmY = {}, tmR = {};
+  if (g.epi_tma) {
+    const int bc = t32_box_c(block_n), box_w = p.tw < 64 ? p.tw : 64;
+    const int64_t px = (int64_t)a->oy_off * a->y.w + a->ox_off;
+    for (int m = 0; m < (a->res.ptr ? 2 : 1); ++m) {
+      const vps_tensor& t = m ? a->res : a->y;
+      cuuint64_t dims[4] = {(cuuint64_t)a->cout, (cuuint64_t)a->ow, (cuuint64_t)a->oh, (cuuint64_t)a->x.n};
+      cuuint64_t strides[3] = {(cuuint64_t)t.cs * 4, (cuuint64_t)a->y.w * t.cs * 4, (cuuint64_t)a->y.h * a->y.w * t.cs * 4};
+      cuuint32_t box[4] = {(cuuint32_t)bc, (cuuint32_t)box_w, (cuuint32_t)(64 / box_w), 1};
+      cuuint32_t estr[4] = {1, 1, 1, 1};
+      CUresult r = encode(m ? &tmR : &tmY, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (float*)t.ptr + px * t.cs, dims, strides, box, estr,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, bc == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (r != CUDA_SUCCESS) { vps::set_error("conv2d_tc32: encode %s failed (%d)", m ? "residual" : "output", (int)r); return VPS_E_CUDA; }
+    }
+  }
+  const int smem = g.a_side + p.b_stages * T32_PLANES * e.b_plane_bytes + (g.epi_tma ? t32_epi_bytes(g.nwg, block_n) : 0) + 1024 +
+                   T32_BAR_BYTES;
+  const auto kernel = g.nwg == 4 ? (g.epi_tma ? conv_igemm_tc32_kernel<4, true> : conv_igemm_tc32_kernel<4, false>)
+                                  : (g.epi_tma ? conv_igemm_tc32_kernel<2, true> : conv_igemm_tc32_kernel<2, false>);
+  static bool smem_set[4] = {false, false, false, false};
+  const int inst = 2 * (g.nwg == 4) + g.epi_tma;
+  if (!smem_set[inst]) {
     if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
       vps::set_error("conv2d_tc32: cannot raise dynamic smem: %s", cudaGetErrorString(cudaGetLastError()));
       return VPS_E_CUDA;
     }
-    smem_set[g.nwg == 4] = true;
+    smem_set[inst] = true;
   }
   const int grid = p.total_tiles < g_num_sms32 ? p.total_tiles : g_num_sms32;
   static int pdl_env = -1;
@@ -764,7 +936,7 @@ extern "C" int vps_conv2d_tc32_multi(const vps_conv_args* args, int nprob, void*
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = pdl_env ? 1 : 0;
-  const cudaError_t le = cudaLaunchKernelEx(&cfg, kernel, tmA, tmB, p, e);
+  const cudaError_t le = cudaLaunchKernelEx(&cfg, kernel, tmA, tmB, tmY, tmR, p, e);
   if (le != cudaSuccess) { vps::set_error("conv2d_tc32: launch failed: %s", cudaGetErrorString(le)); return VPS_E_CUDA; }
   VPS_CUDA_LAST("conv_igemm_tc32_kernel");
   return VPS_OK;
@@ -776,7 +948,7 @@ extern "C" int vps_conv2d_tc32_plan(const vps_conv_args* a, int nprob, int* plan
   Tc32Plan g;
   const int st = tc32_plan(a, nprob, g);
   if (st != VPS_OK) return st;
-  plan[0] = g.nwg; plan[1] = g.block_n; plan[2] = g.tw; plan[3] = g.th; plan[4] = g.halo;
+  plan[0] = g.nwg; plan[1] = g.block_n; plan[2] = g.tw; plan[3] = g.th; plan[4] = g.halo; plan[5] = g.epi_tma;
   return VPS_OK;
 }
 

@@ -146,13 +146,32 @@ __device__ __forceinline__ TileCoord tile_coord(const ConvTcParams& p, int tile)
 }
 
 // ---------------------------------------------------------------- epilogue
-// bias / residual / activation / scale / store of the channel pair (c, c + 1) of output pixel `pix` (c + 1 only if `two`)
-__device__ __forceinline__ void epi_pair(const ConvTcParams& p, float v0, float v1, int64_t pix, int c, bool two) {
-  if (p.bias) {
-    v0 += __ldg(p.bias + c);
-    if (two) v1 += __ldg(p.bias + c + 1);
+// bias / residual / activation / scale of one channel pair (b = bias, r = residual).  Every epilogue goes through this
+// function, so the fp32 operations and their order are the same whichever way the values are loaded and stored.
+__device__ __forceinline__ float2 epi_math(const ConvTcParams& p, float v0, float v1, float b0, float b1, float r0, float r1) {
+  if (p.bias) { v0 += b0; v1 += b1; }
+  if (p.res && !p.res_after_act) { v0 += r0; v1 += r1; }
+  float v[2] = {v0, v1};
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    float t = v[j];
+    if (p.act == VPS_ACT_RELU) t = fmaxf(t, 0.f);
+    else if (p.act == VPS_ACT_LRELU) t = t > 0.f ? t : t * p.slope;
+    else if (p.act == VPS_ACT_SIGMOID) t = 1.f / (1.f + __expf(-t));
+    v[j] = t * p.out_scale;
   }
-  float r0 = 0.f, r1 = 0.f;
+  if (p.res && p.res_after_act) { v[0] += r0; v[1] += r1; }
+  return make_float2(v[0], v[1]);
+}
+
+// bias and residual of the channel pair (c, c + 1) of output pixel `pix` (c + 1 only if `two`)
+__device__ __forceinline__ void epi_load(const ConvTcParams& p, int64_t pix, int c, bool two, float& b0, float& b1, float& r0,
+                                         float& r1) {
+  b0 = b1 = r0 = r1 = 0.f;
+  if (p.bias) {
+    b0 = __ldg(p.bias + c);
+    if (two) b1 = __ldg(p.bias + c + 1);
+  }
   if (p.res) {
     const int64_t ro = pix * p.res_cs + c;       // even element index: pair loads are aligned when res_vec
     if (p.res_dtype == VPS_BF16) {
@@ -174,34 +193,31 @@ __device__ __forceinline__ void epi_pair(const ConvTcParams& p, float v0, float 
         if (two) r1 = rp[1];
       }
     }
-    if (!p.res_after_act) { v0 += r0; v1 += r1; }
-  }
-  float v[2] = {v0, v1};
-#pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    float t = v[j];
-    if (p.act == VPS_ACT_RELU) t = fmaxf(t, 0.f);
-    else if (p.act == VPS_ACT_LRELU) t = t > 0.f ? t : t * p.slope;
-    else if (p.act == VPS_ACT_SIGMOID) t = 1.f / (1.f + __expf(-t));
-    v[j] = t * p.out_scale;
-  }
-  if (p.res && p.res_after_act) { v[0] += r0; v[1] += r1; }
-  const int64_t yo = pix * p.y_cs + c;           // even element index: pair stores are aligned when y_vec
-  if (p.y_dtype == VPS_BF16) {
-    __nv_bfloat16* yp = (__nv_bfloat16*)p.y + yo;
-    if (two && p.y_vec) *reinterpret_cast<__nv_bfloat162*>(yp) = __floats2bfloat162_rn(v[0], v[1]);
-    else { yp[0] = __float2bfloat16_rn(v[0]); if (two) yp[1] = __float2bfloat16_rn(v[1]); }
-  } else {
-    float* yp = (float*)p.y + yo;
-    if (two && p.y_vec) *reinterpret_cast<float2*>(yp) = make_float2(v[0], v[1]);
-    else { yp[0] = v[0]; if (two) yp[1] = v[1]; }
   }
 }
 
-// One consumer warpgroup's m64nN accumulator (rows row0 .. row0 + 63 of the 128-pixel tile) -> NHWC output.  Fragment layout
-// of wgmma: warp w of the group, lane l holds d[4j + 2h + e] = D[16w + l/4 + 8h][8j + 2(l%4) + e].
-template <int N>
+// store of the channel pair (c, c + 1) of output pixel `pix` (c + 1 only if `two`)
+__device__ __forceinline__ void epi_store(const ConvTcParams& p, float2 v, int64_t pix, int c, bool two) {
+  const int64_t yo = pix * p.y_cs + c;           // even element index: pair stores are aligned when y_vec
+  if (p.y_dtype == VPS_BF16) {
+    __nv_bfloat16* yp = (__nv_bfloat16*)p.y + yo;
+    if (two && p.y_vec) *reinterpret_cast<__nv_bfloat162*>(yp) = __floats2bfloat162_rn(v.x, v.y);
+    else { yp[0] = __float2bfloat16_rn(v.x); if (two) yp[1] = __float2bfloat16_rn(v.y); }
+  } else {
+    float* yp = (float*)p.y + yo;
+    if (two && p.y_vec) *reinterpret_cast<float2*>(yp) = v;
+    else { yp[0] = v.x; if (two) yp[1] = v.y; }
+  }
+}
+
+// One consumer warpgroup's m64nN accumulator (rows row0 .. row0 + 63 of the tile) -> NHWC output.  Fragment layout of wgmma:
+// warp w of the group, lane l holds d[4j + 2h + e] = D[16w + l/4 + 8h][8j + 2(l%4) + e].
+// y may alias the bias and the residual as far as the compiler knows, so a load written after a store waits for it.  The
+// loads of PAIRS channel pairs of a row are therefore all issued before any of their stores: one global round trip per
+// group instead of one per pair.  PAIRS is the most the caller's register budget holds without spilling.
+template <int N, int PAIRS>
 __device__ __forceinline__ void epi_frag(const ConvTcParams& p, const float (&d)[N / 2], int tile, int row0) {
+  constexpr int G = N / 8 < PAIRS ? N / 8 : PAIRS;
   const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
   const TileCoord t = tile_coord(p, tile);
   const int nbase = t.n_idx * p.block_n;
@@ -214,9 +230,19 @@ __device__ __forceinline__ void epi_frag(const ConvTcParams& p, const float (&d)
     if (oy >= p.oh || ox >= p.ow) continue;
     const int64_t pix = ((int64_t)t.img * p.y_h + (oy * p.oy_mul + p.oy_off_[t.prob])) * p.y_w + (ox * p.ox_mul + p.ox_off_[t.prob]);
 #pragma unroll
-    for (int j = 0; j < N / 8; ++j) {
-      const int c = nbase + 8 * j + 2 * (lane & 3);
-      if (c < nlim) epi_pair(p, d[4 * j + 2 * h], d[4 * j + 2 * h + 1], pix, c, c + 1 < nlim);
+    for (int j0 = 0; j0 < N / 8; j0 += G) {
+      float b[G][2], r[G][2];
+#pragma unroll
+      for (int j = 0; j < G; ++j) {
+        const int c = nbase + 8 * (j0 + j) + 2 * (lane & 3);
+        if (c < nlim) epi_load(p, pix, c, c + 1 < nlim, b[j][0], b[j][1], r[j][0], r[j][1]);
+      }
+#pragma unroll
+      for (int j = 0; j < G; ++j) {
+        const int c = nbase + 8 * (j0 + j) + 2 * (lane & 3);
+        const int k = 4 * (j0 + j) + 2 * h;
+        if (c < nlim) epi_store(p, epi_math(p, d[k], d[k + 1], b[j][0], b[j][1], r[j][0], r[j][1]), pix, c, c + 1 < nlim);
+      }
     }
   }
 }
