@@ -129,6 +129,12 @@ int vps_tc32_overflow(int reset);
  * x fp32 NHWC (c % 32 == 0), offset fp32 NHWC [..,18], w = vps_pack_weights_tc32 buffer of the [cout,cin,3,3] kernel. */
 int vps_deform_conv_tc32(const vps_tensor* x, const vps_tensor* offset, const void* w, int cout, const vps_tensor* y,
                          void* stream);
+/* The tiling vps_deform_conv_tc32 launches for input x (shape only, no pointer is read) and cout output channels, from the
+ * shapes and the current device's SM count: plan[0] = pixels per tile (128 or 64), plan[1] = output channels per consumer
+ * warpgroup, plan[2] = layout (0 split-M: the two consumer warpgroups take 64 pixels each, the tile has plan[1] channels;
+ * 1 split-N: both take the tile's 64 pixels, the tile has 2 * plan[1] channels), plan[3] = N tiles (each samples the input
+ * again).  `plan` holds 4 ints. */
+int vps_deform_conv_tc32_plan(const vps_tensor* x, int cout, int* plan);
 
 /* explicit im2col for small-cin layers feeding vps_conv2d_tc as a 1x1 conv: cols is NHWC
  * [n, oh, ow, kpad] with k = (r*kw+s)*cin + ci, zero padded to cols.c. */

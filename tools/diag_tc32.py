@@ -112,7 +112,7 @@ def main():
               flush=True)
         del x, y, layer
     if "--dcn" in sys.argv:
-        for (h, w) in [(256, 512), (128, 256), (64, 128)]:
+        for (h, w) in [(256, 512), (128, 256), (64, 128), (32, 64)]:
             for (ci, co) in [(256, 256), (256, 128), (128, 128)]:
                 g = torch.Generator().manual_seed(0)
                 x = torch.randn(1, h, w, ci, generator=g).to(dev)
@@ -122,7 +122,9 @@ def main():
                 y = torch.empty(1, h, w, co, dtype=torch.float32, device=dev)
                 ms = timeit(lambda: ops.deform_conv_tc32(x, off, pk, y), iters)
                 fl = 2.0 * h * w * co * ci * 9
-                print("dcn32 %3d->%3d @%3dx%3d: %.4f ms  %6.1f TF/s alg" % (ci, co, h, w, ms, fl / ms / 1e9), flush=True)
+                plan = ops.deform_conv_tc32_plan(x, pk)
+                print("dcn32 %3d->%3d @%3dx%3d: %.4f ms  %6.1f TF/s alg  %s %d px bn %d, %d N tiles"
+                      % (ci, co, h, w, ms, fl / ms / 1e9, plan["layout"], plan["rows"], plan["bn"], plan["n_tiles"]), flush=True)
 
 
 if __name__ == "__main__":

@@ -69,7 +69,7 @@ EXPORTS = [
     "vps_last_error", "vps_version", "vps_launch_count", "vps_add_launch_count",
     "vps_conv2d_tc", "vps_conv2d_tc_multi", "vps_conv2d_simt", "vps_pack_weights_tc", "vps_pack_weights_simt",
     "vps_packed_tc_bytes", "vps_im2col",
-    "vps_conv2d_tc32", "vps_conv2d_tc32_multi", "vps_conv2d_tc32_plan", "vps_pack_weights_tc32", "vps_packed_tc32_bytes", "vps_tc32_overflow", "vps_deform_conv_tc32",
+    "vps_conv2d_tc32", "vps_conv2d_tc32_multi", "vps_conv2d_tc32_plan", "vps_pack_weights_tc32", "vps_packed_tc32_bytes", "vps_tc32_overflow", "vps_deform_conv_tc32", "vps_deform_conv_tc32_plan",
     "vps_correlation", "vps_correlation_tc", "vps_correlation_simt", "vps_correlation_tc32", "vps_correlation_tc32_ws_bytes", "vps_resample2d", "vps_channelnorm", "vps_flownet_input", "vps_flownet_stage", "vps_flownet_cat3", "vps_flow_deconv",
     "vps_nchw_to_nhwc", "vps_nhwc_to_nchw", "vps_copy_scale", "vps_axpby",
     "vps_space_to_depth2", "vps_tap_gather3x3", "vps_preprocess_u8", "vps_resize_bilinear", "vps_resize_nearest", "vps_pool2d", "vps_groupnorm",

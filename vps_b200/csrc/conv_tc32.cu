@@ -62,6 +62,7 @@ struct Tc32Extra {
   int b_plane_bytes;         // block_n * 64: one weight plane of one step
   int nk_last;               // K16 slabs of the last channel chunk that hold real channels
   int dcn;                   // 1: the operand planes are produced by the deformable-sampling warps (no activation TMA)
+  int dcn_split_n;           // DCN split-N layout: the consumer warpgroups share the tile's pixels, each takes block_n / 2 channels
   int sleep_ns;              // back-off of the converter / producer waits (VPS_TC32_SLEEP, default 0 = poll)
 };
 
@@ -70,14 +71,23 @@ struct Dcn32Params {
   const float* off;
   int x_cs, off_cs, H, W;
 };
-constexpr int DCN32_SETUP_BYTES = 9 * BLOCK_M * 32;      // per (tap, pixel): 4 bilinear weights + 4 element offsets
+constexpr int dcn32_setup_bytes(int rows) { return 9 * rows * 32; }    // per (tap, pixel): 4 bilinear weights + 4 element offsets
 // the fused DCN kernel is bound by its sampling warps (CUDA-core issue + L1 latency), so it runs 4 warpgroups: warp 0 = weight
-// TMA, warps 1-3 and 12-15 = 7 sampling warps, warpgroups 1 and 2 = consumers.  At 128 registers per thread a consumer holds
-// the step accumulator and the promoted sum for N <= 64.
+// TMA, warps 1-3 and 12-15 = 7 sampling warps, warpgroups 1 and 2 = consumers.  setmaxnreg moves registers from warpgroups 0
+// and 3 to the consumers, whose 176 hold the step accumulator and the promoted sum at N = 128 per warpgroup.  Each sample is
+// taken once per tile, so a tile spans every output channel where it can (dcn32_plan):
+//   split-M: 128-pixel tile, warpgroup w takes pixels 64 w .. 64 w + 63 and all bn channels of the tile;
+//   split-N:  64-pixel tile, both warpgroups read the same operand planes, warpgroup w takes channels w bn .. w bn + bn - 1.
 constexpr int DCN32_THREADS = 512;
 constexpr int DCN32_GATHER_WARPS = 7;
-constexpr int DCN32_MAX_N = 64;
-constexpr int DCN32_UNITS_PER_STEP = 16;                 // 8-row x 32-channel units of one K step
+constexpr int DCN32_MAX_N = 128;                         // per consumer warpgroup
+constexpr int DCN32_LO_REGS = 80, DCN32_HI_REGS = 176;   // warpgroups 0, 3 / consumer warpgroups 1, 2
+// __launch_bounds__(512, 1) gives every thread 128 registers: a split asking for more than that pool makes setmaxnreg.inc
+// wait forever
+static_assert(128 * (2 * DCN32_LO_REGS + 2 * DCN32_HI_REGS) == DCN32_THREADS * (65536 / DCN32_THREADS),
+              "the DCN register split must use exactly the launch allocation");
+static_assert(DCN32_LO_REGS % 8 == 0 && DCN32_HI_REGS % 8 == 0 && DCN32_LO_REGS >= 24 && DCN32_HI_REGS <= 256,
+              "setmaxnreg counts are multiples of 8 in [24, 256]");
 
 struct Ring32 {
   uint32_t s_base, s_bytes;      // staging ring
@@ -239,23 +249,25 @@ __device__ __forceinline__ void converter32(const ConvTcParams& p, const Tc32Ext
 // group: column (tap k, channel c) of output pixel (y, x) = bilinear sample of x[c] at (y - 1 + k/3 + dy_k, x - 1 + k%3 + dx_k),
 // zero outside (-1, H) x (-1, W), corner taps outside the image contribute 0.  The sampled fp32 value is split into the two
 // fp16 planes straight into the operand ring -- the 9x column matrix (1.2 GB per P2 layer in fp32) never exists.  K steps run
-// chunk-major / tap-minor: the nine taps of a 32-channel chunk re-read the same few KB of input from L1.
+// chunk-major / tap-minor: the nine taps of a 32-channel chunk re-read the same few KB of input from L1.  A tile has e.rows
+// (128 or 64) pixels, i.e. e.rows / 8 sampling units per K step.
 __device__ __forceinline__ void dcn_gather32(const ConvTcParams& p, const Tc32Extra& e, const Dcn32Params& d, const Ring32& rg,
                                              uint32_t setup_base, uint32_t ctr_addr, int gtid) {
   constexpr int NT = 32 * DCN32_GATHER_WARPS;
   const int H = d.H, W = d.W;
   const int lane = gtid & 31;
   const int j = lane & 3;                    // 8-channel group of the 32-channel chunk
+  const int rlog = e.rows == 128 ? 7 : 6, ulog = rlog - 3;
   const int steps_per_tile = p.cin_chunks * 9;
-  const uint32_t units_per_tile = (uint32_t)steps_per_tile * 16u;      // a unit = 8 rows (pixels) x 32 channels of one K step
+  const uint32_t units_per_tile = (uint32_t)steps_per_tile << ulog;   // a unit = 8 rows (pixels) x 32 channels of one K step
   const uint32_t a_stages = (uint32_t)p.a_stages;
   uint32_t step_base = 0;                    // K steps of the tiles this CTA has finished
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const TileCoord t = tile_coord(p, tile);
     if (gtid == 0) asm volatile("st.volatile.shared.u32 [%0], %1;" ::"r"(ctr_addr), "r"(0u) : "memory");
     // ---- sampling set-up of all (tap, pixel) pairs of this tile
-    for (int item = gtid; item < 9 * BLOCK_M; item += NT) {
-      const int k = item >> 7, r = item & (BLOCK_M - 1);
+    for (int item = gtid; item < 9 << rlog; item += NT) {
+      const int k = item >> rlog, r = item & ((1 << rlog) - 1);
       const int ty_in = r / p.tw, tx_in = r - ty_in * p.tw;
       const int yo = t.ty * p.th + ty_in, xo = t.tx * p.tw + tx_in;
       float wts[4] = {0.f, 0.f, 0.f, 0.f};
@@ -283,13 +295,13 @@ __device__ __forceinline__ void dcn_gather32(const ConvTcParams& p, const Tc32Ex
     }
     asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory");
     // ---- units are claimed dynamically (any number of gather warps stays balanced; a warp may run ahead into the next
-    //      K step's ring slot): unit u = (K step u / 16, rows 8 * (u % 16) ..), K steps chunk-major / tap-minor
+    //      K step's ring slot): unit u = (K step u / units, rows 8 * (u % units) ..), K steps chunk-major / tap-minor
     while (true) {
       uint32_t u = 0;
       if (lane == 0) asm volatile("atom.shared.add.u32 %0, [%1], 1;" : "=r"(u) : "r"(ctr_addr) : "memory");
       u = __shfl_sync(0xffffffffu, u, 0);
       if (u >= units_per_tile) break;
-      const uint32_t step = u >> 4, part = u & 15u;
+      const uint32_t step = u >> ulog, part = u & ((1u << ulog) - 1u);
       const uint32_t cc = step / 9u, k = step - cc * 9u;
       const uint32_t sg = step_base + step;             // K step counted over all tiles of this CTA -> ring slot and its use count
       const uint32_t use = sg / a_stages, as = sg - use * a_stages;
@@ -298,7 +310,7 @@ __device__ __forceinline__ void dcn_gather32(const ConvTcParams& p, const Tc32Ex
       const int r = (int)(part * 8u) + (lane >> 2);
       const float* xc = d.x + cc * T32_KC + j * 8;
       {
-        const uint32_t sa = setup_base + (uint32_t)(k * BLOCK_M + r) * 32u;
+        const uint32_t sa = setup_base + (uint32_t)((k << rlog) + r) * 32u;
         float wq[4];
         int oq[4];
         asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(wq[0]), "=f"(wq[1]), "=f"(wq[2]), "=f"(wq[3]) : "r"(sa));
@@ -330,7 +342,7 @@ __device__ __forceinline__ void dcn_gather32(const ConvTcParams& p, const Tc32Ex
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy writes -> tensor-core reads
       __syncwarp();
-      if (lane == 0) mbar_arrive(rg.pfull((int)as));                   // 16 warp-units complete a K step's operand planes
+      if (lane == 0) mbar_arrive(rg.pfull((int)as));                   // e.rows / 8 warp-units complete a K step's operand planes
     }
     step_base += (uint32_t)steps_per_tile;
     asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory");      // the set-up table and the unit counter are rewritten for the next tile
@@ -405,9 +417,11 @@ __device__ __forceinline__ void epi_tma32(const ConvTcParams& p, const CUtensorM
 // and weight tiles of the step are released as soon as its MMAs have completed (one arrival per consumer warpgroup).
 // With the TMA epilogue the leader loads the tile's residual boxes after the first K step: by then the previous tile's store
 // has long read the boxes, so its wait does not hold up the first MMAs.
+// The warpgroup's share of the tile: pixels row0 .. row0 + 63, the N weight rows from byte b_off of each weight plane, tile
+// channels c_off .. c_off + N - 1 (the convolution: 64 wg, 0, 0).
 template <int N, bool TMA_EPI>
-__device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, int wg,
-                                           const CUtensorMap* tmY, const CUtensorMap* tmR) {
+__device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, int wg, int row0,
+                                           uint32_t b_off, int c_off, const CUtensorMap* tmY, const CUtensorMap* tmR) {
   constexpr int BC = t32_box_c(N);
   const bool leader = (threadIdx.x & 127) == 0;
   constexpr bool epi_tma = TMA_EPI;
@@ -418,8 +432,8 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
   const int ntaps = p.kh * p.kw, kw = p.kw, last_cc = p.cin_chunks - 1;
   const uint32_t a_pitch = halo ? (uint32_t)p.halo_w * 64u : 512u;      // byte distance of the A planes' 8-row groups
   const uint64_t a_hi = desc_hi(64u, a_pitch), b_hi = desc_hi(64u, 512u);
-  // this warpgroup's 64 pixels: 8 halo rows (of 8 tile pixels each) down, or 64 dense rows
-  const uint32_t a_wg = halo ? (uint32_t)wg * 8u * a_pitch : (uint32_t)wg * 64u * 64u;
+  // this warpgroup's 64 pixels: row0 / 8 halo rows (of 8 tile pixels each) down, or row0 dense rows
+  const uint32_t a_wg = halo ? (uint32_t)(row0 >> 3) * a_pitch : (uint32_t)row0 * 64u;
   const uint32_t plane = (uint32_t)e.plane_bytes, b_plane = (uint32_t)e.b_plane_bytes;
   float acc[N / 2], sum[N / 2];
   int as = 0, bs = 0;
@@ -443,7 +457,7 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
         }
         mbar_wait(rg.bfull(bs), bphase);
         const uint32_t a_addr = halo ? a_item + (uint32_t)r * a_pitch + (uint32_t)s * 64u : a_item;
-        const uint32_t b_addr = rg.b_base + bs * rg.b_bytes;
+        const uint32_t b_addr = rg.b_base + bs * rg.b_bytes + b_off;
         const uint64_t A = desc_at(a_hi, a_addr), A2 = desc_at(a_hi, a_addr + plane);
         const uint64_t B = desc_at(b_hi, b_addr), B2 = desc_at(b_hi, b_addr + b_plane);
         wg::fence();
@@ -490,7 +504,7 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
       epi_tma32<N>(p, tmY, sum, box, bias_s, bias_v, rbar, rphase, wg, tile);
       if (p.res) rphase ^= 1u;
     } else {
-      epi_frag<N, 4>(p, sum, tile, wg * 64);
+      epi_frag<N, 4>(p, sum, tile, row0, c_off);
     }
   }
   // the boxes must stay allocated until the last store has read them, and the stores must be complete before the grid is
@@ -502,11 +516,11 @@ template <int NWG, bool TMA_EPI>
 __device__ __forceinline__ void consumer32_n(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, int wg,
                                              const CUtensorMap* tmY, const CUtensorMap* tmR) {
   switch (p.block_n) {
-    case 16: consumer32<16, TMA_EPI>(p, e, rg, wg, tmY, tmR); break;
-    case 32: consumer32<32, TMA_EPI>(p, e, rg, wg, tmY, tmR); break;
-    case 64: consumer32<64, TMA_EPI>(p, e, rg, wg, tmY, tmR); break;
+    case 16: consumer32<16, TMA_EPI>(p, e, rg, wg, 64 * wg, 0u, 0, tmY, tmR); break;
+    case 32: consumer32<32, TMA_EPI>(p, e, rg, wg, 64 * wg, 0u, 0, tmY, tmR); break;
+    case 64: consumer32<64, TMA_EPI>(p, e, rg, wg, 64 * wg, 0u, 0, tmY, tmR); break;
     default:
-      if constexpr (NWG == 2 && !TMA_EPI) consumer32<T32_MAX_N, false>(p, e, rg, wg, tmY, tmR);
+      if constexpr (NWG == 2 && !TMA_EPI) consumer32<T32_MAX_N, false>(p, e, rg, wg, 64 * wg, 0u, 0, tmY, tmR);
       else __trap();                      // the host plan pairs block_n > T32_EPI_MAX_N with neither NWG = 4 nor the TMA epilogue
       break;
   }
@@ -568,22 +582,29 @@ dcn_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmB, const ConvTcParam
   rg.a_base = smem_base; rg.a_bytes = (uint32_t)T32_PLANES * (uint32_t)e.plane_bytes;
   rg.b_base = rg.a_base + (uint32_t)p.a_stages * rg.a_bytes; rg.b_bytes = (uint32_t)T32_PLANES * (uint32_t)e.b_plane_bytes;
   const uint32_t setup_base = rg.b_base + (uint32_t)p.b_stages * rg.b_bytes;
-  rg.bar_base = setup_base + DCN32_SETUP_BYTES;
+  rg.bar_base = setup_base + dcn32_setup_bytes(e.rows);
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);     // warp-uniform role index (wgmma issue is not treated as divergent)
-  if (warp == 0) init_bars32(rg, DCN32_UNITS_PER_STEP, 1, 2);
+  if (warp == 0) init_bars32(rg, (uint32_t)e.rows / 8u, 1, 2);
   if (threadIdx.x == 32) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
   __syncthreads();
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (warp >= 4 && warp < 12) {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(DCN32_HI_REGS));
     const int wg = (warp - 4) >> 2;
-    if (p.block_n == 16) consumer32<16, false>(p, e, rg, wg, nullptr, nullptr);
-    else if (p.block_n == 32) consumer32<32, false>(p, e, rg, wg, nullptr, nullptr);
-    else consumer32<DCN32_MAX_N, false>(p, e, rg, wg, nullptr, nullptr);
-  } else if (warp == 0) {
-    producer32(p, e, rg, &tmB, &tmB);
+    const int bn = e.dcn_split_n ? p.block_n / 2 : p.block_n;
+    const int row0 = e.dcn_split_n ? 0 : 64 * wg, c_off = e.dcn_split_n ? bn * wg : 0;
+    const uint32_t b_off = (uint32_t)c_off * 64u;       // 64-byte weight rows
+    switch (bn) {
+      case 16: consumer32<16, false>(p, e, rg, wg, row0, b_off, c_off, nullptr, nullptr); break;
+      case 32: consumer32<32, false>(p, e, rg, wg, row0, b_off, c_off, nullptr, nullptr); break;
+      case 64: consumer32<64, false>(p, e, rg, wg, row0, b_off, c_off, nullptr, nullptr); break;
+      default: consumer32<DCN32_MAX_N, false>(p, e, rg, wg, row0, b_off, c_off, nullptr, nullptr); break;
+    }
   } else {
-    dcn_gather32(p, e, d, rg, setup_base, rg.unit_ctr(), warp < 4 ? (int)threadIdx.x - 32 : (int)threadIdx.x - 384 + 96);
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(DCN32_LO_REGS));
+    if (warp == 0) producer32(p, e, rg, &tmB, &tmB);
+    else dcn_gather32(p, e, d, rg, setup_base, rg.unit_ctr(), warp < 4 ? (int)threadIdx.x - 32 : (int)threadIdx.x - 384 + 96);
   }
 }
 
@@ -757,6 +778,74 @@ int tc32_plan(const vps_conv_args* a, int nprob, Tc32Plan& out) {
   }
   const int bst = (T32_SMEM_BUDGET - out.a_side - (out.epi_tma ? eb : 0)) / (T32_PLANES * out.block_n * 64);
   out.b_stages = bst > MAX_STAGES ? MAX_STAGES : bst;
+  return VPS_OK;
+}
+
+// Tiling of one fused DCN launch.  Everything follows from the shapes (and the SM count); vps_deform_conv_tc32 launches exactly
+// this plan and vps_deform_conv_tc32_plan reports it.
+struct Dcn32Plan {
+  int rows;                  // tile pixels: 128 (split-M) or 64 (split-N)
+  int split_n;
+  int bn;                    // channels per consumer warpgroup
+  int block_n;               // channels per tile: bn (split-M) or 2 bn (split-N)
+  int n_tiles;               // cout_pad / block_n
+  int tw, th;
+  int a_stages, b_stages, smem;
+};
+// Shared memory stays at most 132 KB so that L1 keeps room: the sampling warps read 4 x 128 B per (tap, pixel, 32-channel
+// chunk) through L1, and the nine taps of a chunk re-read the same ~60 KB footprint of the tile.
+constexpr int DCN32_SMEM_MAX = 132 * 1024;
+// Clocks of the CTA's 7 sampling warps per 8-pixel x 32-channel unit, from per-layer H100 timings of the 128-pixel x 64
+// tiling (DESIGN.md §5.0: about 120 ns at every layer and level; the units are latency bound, 7 in flight per CTA), and the
+// latency floor of a consumer K step (two dependent wgmma round trips, as in tc32_plan).
+constexpr double DCN32_UNIT_CLK = 220.0, DCN32_STEP_CLK = 300.0;
+
+// (layout, bn) minimising waves * (K steps * step clocks + epilogue), among those whose tile width divides cout_pad and whose
+// rings fit.  A K step costs the larger of: the sampling of rows / 8 units; the consumers' latency floor or their 12 MMAs of
+// m64 x bn x k16 (6 bn clocks of the tensor pipe); the weight tile (2 planes x block_n x 64 B) at the L2 rate of 56 B/clk.
+// Every N tile samples the same input again, so a tile as wide as cout_pad samples each input once; narrower tiles win where
+// the grid would otherwise leave SMs idle.  Equal costs go to the plan that samples less.
+int dcn32_plan(int n, int h, int w, int cin, int cout, Dcn32Plan& out) {
+  const int sms = num_sms32();
+  if (sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
+  const int cout_pad = (cout + 15) / 16 * 16;
+  const int steps = cin / T32_KC * 9;
+  double best = -1.0, best_units = 0.0;
+  for (int split_n = 0; split_n <= 1; ++split_n) {
+    const int rows = split_n ? 64 : 128;
+    int best_tw = 16; int64_t best_area = -1;
+    const int cands[5] = {16, 8, 32, 64, 128};
+    for (int i = 0; i < 5; ++i) {
+      const int tw = cands[i], th = rows / tw;
+      if (th == 0) continue;
+      const int64_t area = (int64_t)vps::cdiv(w, tw) * tw * vps::cdiv(h, th) * th;
+      if (best_area < 0 || area < best_area) { best_area = area; best_tw = tw; }
+    }
+    const int64_t m_tiles = (int64_t)n * vps::cdiv(h, rows / best_tw) * vps::cdiv(w, best_tw);
+    const int a_side = 2 * T32_PLANES * rows * 64 + dcn32_setup_bytes(rows);
+    for (int bn = 16; bn <= DCN32_MAX_N; bn *= 2) {
+      const int block_n = split_n ? 2 * bn : bn;
+      if (block_n > cout_pad || cout_pad % block_n) continue;
+      const int b_slot = T32_PLANES * block_n * 64;
+      const int bst = (DCN32_SMEM_MAX - 1024 - T32_BAR_BYTES - a_side) / b_slot;
+      if (bst < 2) continue;
+      const int64_t tiles = m_tiles * (cout_pad / block_n);
+      const double waves = (double)((tiles + sms - 1) / sms);
+      const double step = fmax(fmax(rows / 8 * DCN32_UNIT_CLK, fmax(DCN32_STEP_CLK, 6.0 * bn)), b_slot / 56.0);
+      const double t = waves * ((double)steps * step + 40.0 * bn + 1500.0), units = waves * rows;
+      if (best < 0 || t < best * 0.999 || (t <= best * 1.001 && units < best_units)) {
+        best = t; best_units = units;
+        out.rows = rows; out.split_n = split_n; out.bn = bn; out.block_n = block_n; out.n_tiles = cout_pad / block_n;
+        out.tw = best_tw; out.th = rows / best_tw;
+        out.a_stages = 2; out.b_stages = bst > 3 ? 3 : bst;
+        out.smem = a_side + out.b_stages * b_slot + 1024 + T32_BAR_BYTES;
+      }
+    }
+  }
+  if (best < 0) {
+    vps::set_error("deform_conv_tc32: no tiling fits (cout %d)", cout);
+    return VPS_E_ARG;
+  }
   return VPS_OK;
 }
 
@@ -967,43 +1056,26 @@ extern "C" int vps_deform_conv_tc32(const vps_tensor* x, const vps_tensor* offse
   VPS_CHECK_ARG(((uintptr_t)w & 127) == 0, "deform_conv_tc32: weights not aligned");
   auto encode = get_encode32();
   if (!encode) { vps::set_error("cuTensorMapEncodeTiled unavailable"); return VPS_E_CUDA; }
-  if (num_sms32() <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
+  VPS_CHECK_ARG(y->dtype == VPS_F32, "deform_conv_tc32: y must be fp32");
+  Dcn32Plan g;
+  const int st = dcn32_plan(x->n, x->h, x->w, x->c, cout, g);
+  if (st != VPS_OK) return st;
   const int cout_pad = (cout + 15) / 16 * 16;
   ConvTcParams p = {};
   Tc32Extra e = {};
   p.bk = T32_KC; p.nprob = 1;
   p.n_img = x->n; p.oh = x->h; p.ow = x->w;
-  int best_tw = 16; int64_t best_area = -1;
-  const int cands[5] = {16, 8, 32, 64, 128};
-  for (int i = 0; i < 5; ++i) {
-    const int tw = cands[i], th = 128 / tw;
-    const int64_t area = (int64_t)vps::cdiv(x->w, tw) * tw * vps::cdiv(x->h, th) * th;
-    if (best_area < 0 || area < best_area) { best_area = area; best_tw = tw; }
-  }
-  p.tw = best_tw; p.th = 128 / best_tw;
+  p.tw = g.tw; p.th = g.th;
   p.tiles_x = vps::cdiv(x->w, p.tw); p.tiles_y = vps::cdiv(x->h, p.th);
-  const int block_n = cout_pad % DCN32_MAX_N == 0 ? DCN32_MAX_N : (cout_pad % 32 == 0 ? 32 : 16);
-  p.block_n = block_n; p.n_tiles_n = cout_pad / block_n;
+  const int block_n = g.block_n;
+  p.block_n = block_n; p.n_tiles_n = g.n_tiles;
   p.kh = p.kw = 3; p.sh = p.sw = 1; p.halo = 0; p.halo_w = 0;
   p.cin_chunks = x->c / T32_KC;
-  e.rows = BLOCK_M; e.dcn = 1;
-  e.plane_bytes = BLOCK_M * 64; e.stage_bytes = 0; e.nk_last = 2;
+  e.rows = g.rows; e.dcn = 1; e.dcn_split_n = g.split_n;
+  e.plane_bytes = g.rows * 64; e.stage_bytes = 0; e.nk_last = 2;
   e.b_plane_bytes = block_n * 64;
   p.a_box_bytes = 0; p.a_stage_bytes = T32_PLANES * e.plane_bytes;
-  // Shared memory is kept small on purpose so that L1 keeps room: the sampling warps read 4 x 128 B per (tap, pixel,
-  // 32-channel chunk) through L1, and the nine taps of a chunk re-read the same ~60 KB footprint of the tile.
-  VPS_CHECK_ARG(y->dtype == VPS_F32, "deform_conv_tc32: y must be fp32");
-  static int dcn_a_env = -1, dcn_b_env = -1;
-  if (dcn_a_env < 0) { const char* ev = getenv("VPS_DCN32_A_STAGES"); dcn_a_env = ev ? atoi(ev) : 2; }
-  if (dcn_b_env < 0) { const char* ev = getenv("VPS_DCN32_B_STAGES"); dcn_b_env = ev ? atoi(ev) : 3; }
-  p.a_stages = dcn_a_env < 2 ? 2 : (dcn_a_env > 3 ? 3 : dcn_a_env);
-  {
-    const int budget = 227 * 1024 - 1024 - T32_BAR_BYTES - 64 - DCN32_SETUP_BYTES - p.a_stages * p.a_stage_bytes;
-    int bst = budget / (T32_PLANES * e.b_plane_bytes);
-    p.b_stages = bst > MAX_STAGES ? MAX_STAGES : bst;
-    if (p.b_stages > dcn_b_env && dcn_b_env >= 2) p.b_stages = dcn_b_env;
-    VPS_CHECK_ARG(p.b_stages >= 2, "deform_conv_tc32: ring does not fit");
-  }
+  p.a_stages = g.a_stages; p.b_stages = g.b_stages;
   p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
   p.total_tiles = p.tiles_per_prob;
   p.y = y->ptr; p.y_h = y->h; p.y_w = y->w; p.y_cs = y->cs; p.y_dtype = y->dtype;
@@ -1027,15 +1099,15 @@ extern "C" int vps_deform_conv_tc32(const vps_tensor* x, const vps_tensor* offse
                         CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { vps::set_error("deform_conv_tc32: encode B failed (%d)", (int)r); return VPS_E_CUDA; }
   }
-  const int smem = p.a_stages * p.a_stage_bytes + p.b_stages * T32_PLANES * e.b_plane_bytes + DCN32_SETUP_BYTES + 1024 + T32_BAR_BYTES;
+  const int smem = g.smem;
   static bool smem_set = false;
   if (!smem_set) {
     if (cudaFuncSetAttribute(dcn_igemm_tc32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
       vps::set_error("deform_conv_tc32: cannot raise dynamic smem: %s", cudaGetErrorString(cudaGetLastError()));
       return VPS_E_CUDA;
     }
-    // a hint only: the driver picks the smallest carve-out that holds the launch's dynamic shared memory
-    cudaFuncSetAttribute(dcn_igemm_tc32_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, smem <= 132 * 1024 ? 58 : 100);
+    // a hint only: the driver picks the smallest carve-out that holds the launch's dynamic shared memory (<= DCN32_SMEM_MAX)
+    cudaFuncSetAttribute(dcn_igemm_tc32_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 58);
     (void)cudaGetLastError();
     smem_set = true;
   }
@@ -1050,5 +1122,14 @@ extern "C" int vps_deform_conv_tc32(const vps_tensor* x, const vps_tensor* offse
   const cudaError_t le = cudaLaunchKernelEx(&cfg, dcn_igemm_tc32_kernel, tmB, p, e, d);
   if (le != cudaSuccess) { vps::set_error("deform_conv_tc32: launch failed: %s", cudaGetErrorString(le)); return VPS_E_CUDA; }
   VPS_CUDA_LAST("dcn_igemm_tc32_kernel");
+  return VPS_OK;
+}
+
+extern "C" int vps_deform_conv_tc32_plan(const vps_tensor* x, int cout, int* plan) {
+  VPS_CHECK_ARG(x->c % T32_KC == 0 && x->c > 0 && cout > 0, "deform_conv_tc32_plan: cin %d, cout %d", x->c, cout);
+  Dcn32Plan g;
+  const int st = dcn32_plan(x->n, x->h, x->w, x->c, cout, g);
+  if (st != VPS_OK) return st;
+  plan[0] = g.rows; plan[1] = g.bn; plan[2] = g.split_n; plan[3] = g.n_tiles;
   return VPS_OK;
 }

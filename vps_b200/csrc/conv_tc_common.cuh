@@ -210,18 +210,19 @@ __device__ __forceinline__ void epi_store(const ConvTcParams& p, float2 v, int64
   }
 }
 
-// One consumer warpgroup's m64nN accumulator (rows row0 .. row0 + 63 of the tile) -> NHWC output.  Fragment layout of wgmma:
+// One consumer warpgroup's m64nN accumulator (rows row0 .. row0 + 63, channels c_off .. c_off + N - 1 of the tile) -> NHWC
+// output.  Fragment layout of wgmma:
 // warp w of the group, lane l holds d[4j + 2h + e] = D[16w + l/4 + 8h][8j + 2(l%4) + e].
 // y may alias the bias and the residual as far as the compiler knows, so a load written after a store waits for it.  The
 // loads of PAIRS channel pairs of a row are therefore all issued before any of their stores: one global round trip per
 // group instead of one per pair.  PAIRS is the most the caller's register budget holds without spilling.
 template <int N, int PAIRS>
-__device__ __forceinline__ void epi_frag(const ConvTcParams& p, const float (&d)[N / 2], int tile, int row0) {
+__device__ __forceinline__ void epi_frag(const ConvTcParams& p, const float (&d)[N / 2], int tile, int row0, int c_off = 0) {
   constexpr int G = N / 8 < PAIRS ? N / 8 : PAIRS;
   const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
   const TileCoord t = tile_coord(p, tile);
-  const int nbase = t.n_idx * p.block_n;
-  const int nlim = min(p.cout, nbase + p.block_n);
+  const int nbase = t.n_idx * p.block_n + c_off;
+  const int nlim = min(p.cout, nbase + N);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int row = row0 + 16 * w + (lane >> 2) + 8 * h;

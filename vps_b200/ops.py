@@ -446,6 +446,15 @@ def deform_conv_tc32(x, offset, pw, y):
     return y
 
 
+def deform_conv_tc32_plan(x, pw):
+    """The tiling deform_conv_tc32 picks for input x and the layer pw: dict(rows=pixels per tile (128 or 64), bn=output
+    channels per consumer warpgroup, layout="split_m" (each warpgroup takes 64 of the tile's pixels and all bn channels) or
+    "split_n" (both take the tile's 64 pixels, warpgroup w channels w*bn ..), n_tiles=N tiles, each sampling the input again)."""
+    plan = (C.c_int * 4)()
+    check(_real_lib().vps_deform_conv_tc32_plan(_bt(x), pw.cout, plan), "deform_conv_tc32_plan")
+    return dict(rows=plan[0], bn=plan[1], layout="split_n" if plan[2] else "split_m", n_tiles=plan[3])
+
+
 # ------------------------------------------------------------------ detection
 def roi_align(feats, strides, rois, nroi, out, sample_num=2, nroi_dev=None):
     arr = (VpsTensor * len(feats))(*[vt(f) for f in feats])
