@@ -1,5 +1,5 @@
 """Time a list of the step's convolution shapes through vps_conv2d_tc (median of N, L2 flushed between runs).
-Usage: python tools/bench_convs.py [--iters N] [--set small|all]      (VPS_CONV_HALO=0/1/2 selects the A-operand mode)"""
+Usage: python tools/bench_convs.py [--iters N] [--set small|all]"""
 import os
 import sys
 
@@ -50,4 +50,4 @@ for cin, cout, h, w, k, s in SHAPES:
     fl = 2.0 * n * y.shape[1] * y.shape[2] * cout * cin * k * k
     tot += ms
     print("conv %dx%d s%d %4d->%4d @%4dx%4d n%3d: %.4f ms  %7.1f TFLOP/s" % (k, k, s, cin, cout, y.shape[1], y.shape[2], n, ms, fl / ms / 1e9))
-print("total %.3f ms (halo mode %s)" % (tot, os.environ.get("VPS_CONV_HALO", "auto")))
+print("total %.3f ms" % tot)

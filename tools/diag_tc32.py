@@ -1,6 +1,5 @@
 """Per-layer diagnosis of the tc32 convolution kernels: median CUDA-event time with an L2 flush between calls, algorithmic
-TFLOP/s, and the bytes the layer must move (fp32 in + out + residual) against the HBM copy peak.  With VPS_CONV_STATS=1 in the
-environment every launch also prints its per-role barrier-wait clocks (conv_tc32.cu).
+TFLOP/s, and the bytes the layer must move (fp32 in + out + residual) against the HBM copy peak.
 
     python tools/diag_tc32.py [--dcn] [--only SUBSTR]
 """
@@ -69,7 +68,6 @@ def main():
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     only = sys.argv[sys.argv.index("--only") + 1] if "--only" in sys.argv else None
     ops.F32_TC[0] = True
-    iters = 1 if os.environ.get("VPS_CONV_STATS") else 5
     for (n, cin, cout, oh, ow, k, s, res, note) in SHAPES:
         if only and only not in note:
             continue
@@ -89,7 +87,7 @@ def main():
         f = lambda: ops.conv2d(x, pk, y, stride=s, pad=pad, act=ops.ACT_RELU, res=r, use_tc=True, oh=oh, ow=ow)
         plan = ops.conv2d_tc32_plan(x, pk, stride=s, pad=pad, oh=oh, ow=ow, y=y, res=r)
         sys.stderr.flush()
-        ms = timeit(f, iters)
+        ms = timeit(f)
         fl = 2.0 * n * oh * ow * cout * cin * k * k
         by = 4.0 * n * (h * w * cin + oh * ow * cout * (2 if res else 1))
         print("%-28s %dx%d s%d %4d->%4d @%dx%d n%d: %.4f ms  %6.1f TF/s alg  %6.1f MB  hbm-floor %.4f ms (%.2f of it)  "
@@ -106,7 +104,7 @@ def main():
         layer = deconv4x4_s2((torch.randn(cin, cout, 4, 4, generator=g) / (cin * 4) ** 0.5).to(dev),
                              torch.randn(cout, generator=g).to(dev))
         y = empty_nhwc(n, 2 * h, 2 * w, cout, torch.float32, dev)
-        ms = timeit(lambda: layer(x, y, act=ops.ACT_LRELU), iters)
+        ms = timeit(lambda: layer(x, y, act=ops.ACT_LRELU))
         fl = 2.0 * n * h * w * cout * cin * 16
         print("%-28s 2x2 x4 phases %4d->%4d @%dx%d n%d: %.4f ms  %6.1f TF/s alg" % (note, cin, cout, h, w, n, ms, fl / ms / 1e9),
               flush=True)
@@ -120,7 +118,7 @@ def main():
                 wt = (torch.randn(co, ci, 3, 3, generator=g) / (ci * 9) ** 0.5).to(dev)
                 pk = ops.PackedConv(wt, None)
                 y = torch.empty(1, h, w, co, dtype=torch.float32, device=dev)
-                ms = timeit(lambda: ops.deform_conv_tc32(x, off, pk, y), iters)
+                ms = timeit(lambda: ops.deform_conv_tc32(x, off, pk, y))
                 fl = 2.0 * h * w * co * ci * 9
                 plan = ops.deform_conv_tc32_plan(x, pk)
                 print("dcn32 %3d->%3d @%3dx%3d: %.4f ms  %6.1f TF/s alg  %s %d px bn %d, %d N tiles"

@@ -1,6 +1,7 @@
 // Shared device/host helpers for libvps_b200.so (sm_90a).
 #pragma once
 #include <cuda.h>
+#include <cudaTypedefs.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -12,6 +13,15 @@ namespace vps {
 
 void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
+// SM count of the current device (cached; 0 without a device)
+int num_sms();
+// the driver's cuTensorMapEncodeTiled (cached; nullptr, with the error set, if the driver lacks it)
+PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder();
+// Tensor map over the NHWC tensor t: dims {c, w, h, n}, box {box_c, box_w, box_h, 1} read every {1, sw, sh, 1} elements,
+// no interleave or OOB NaN fill.  The pixel, row and image strides come from `strides` (default t): cs, w * cs and h * w * cs
+// elements of type `type` (fp32 or a 16-bit type).  On failure the error, prefixed by `who`, is set and false returned.
+bool encode_nhwc(CUtensorMap* m, const vps_tensor& t, CUtensorMapDataType type, int box_c, int box_w, int box_h, int sw, int sh,
+                 CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2, const char* who, const vps_tensor* strides = nullptr);
 
 #define VPS_CHECK_ARG(cond, ...)          \
   do {                                    \

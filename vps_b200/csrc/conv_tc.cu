@@ -35,17 +35,16 @@ struct Ring {
 };
 
 // ---- halo mode: one activation box per channel chunk (A ring), weights per tap or per filter row (B ring)
-template <bool ROWG, bool STATS>
+template <bool ROWG>
 __device__ __forceinline__ void producer_halo(const ConvTcParams& p, const Ring& rg, const CUtensorMap* tmA,
                                               const CUtensorMap* tmB0, const CUtensorMap* tmB1, const CUtensorMap* tmB2,
-                                              const CUtensorMap* tmB3, int lane) {
+                                              const CUtensorMap* tmB3) {
   const int bk = p.bk, kw = p.kw, cin_chunks = p.cin_chunks, a_stages = p.a_stages, b_stages = p.b_stages;
   const int ngrp = ROWG ? p.kh : p.kh * p.kw;
   const int tiles_per_img = p.tiles_y * p.tiles_x;
   const uint32_t a_box_bytes = (uint32_t)p.a_box_bytes;
   int as = 0, bs = 0;
   uint32_t aphase = 0, bphase = 0;
-  long long st_a = 0, st_b = 0;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const int prob = tile / p.tiles_per_prob;
     const int t_in = tile - prob * p.tiles_per_prob;
@@ -59,18 +58,14 @@ __device__ __forceinline__ void producer_halo(const ConvTcParams& p, const Ring&
     const int n0 = n_idx * p.block_n;
     const CUtensorMap* tmB = prob == 0 ? tmB0 : (prob == 1 ? tmB1 : (prob == 2 ? tmB2 : tmB3));
     for (int cc = 0; cc < cin_chunks; ++cc) {
-      const long long t0 = STATS ? clock64() : 0;
       mbar_wait(rg.aempty(as), aphase ^ 1);
-      if (STATS) st_a += clock64() - t0;
       if (elect_one()) {
         mbar_expect_tx(rg.afull(as), a_box_bytes);
         tma_load_4d(rg.a_base + as * rg.a_stage_bytes, tmA, rg.afull(as), cc * bk, x_base, y_base, img);
       }
       if (++as == a_stages) { as = 0; aphase ^= 1; }
       for (int g = 0; g < ngrp; ++g) {
-        const long long t1 = STATS ? clock64() : 0;
         mbar_wait(rg.bempty(bs), bphase ^ 1);
-        if (STATS) st_b += clock64() - t1;
         if (elect_one()) {
           mbar_expect_tx(rg.bfull(bs), rg.b_stage_bytes);
           tma_load_3d(rg.b_base + bs * rg.b_stage_bytes, tmB, rg.bfull(bs), cc * bk, n0, ROWG ? g * kw : g);
@@ -79,15 +74,13 @@ __device__ __forceinline__ void producer_halo(const ConvTcParams& p, const Ring&
       }
     }
   }
-  if (STATS && lane == 0) { p.stats[blockIdx.x * 8 + 0] = st_a; p.stats[blockIdx.x * 8 + 1] = st_b; }
 }
 
 // ---- flat mode (strided / 1x1 convolutions): K steps in (chunk, tap) order, gsub steps share one ring slot and one
 // barrier round (both operands arrive on the slot's `afull` barrier; the B barriers are unused)
-template <bool STATS>
 __device__ __forceinline__ void producer_flat(const ConvTcParams& p, const Ring& rg, const CUtensorMap* tmA,
                                               const CUtensorMap* tmB0, const CUtensorMap* tmB1, const CUtensorMap* tmB2,
-                                              const CUtensorMap* tmB3, int lane) {
+                                              const CUtensorMap* tmB3) {
   const int bk = p.bk, kw = p.kw, kh = p.kh, stages = p.a_stages, G = p.gsub;
   const int T = p.cin_chunks * kh * kw;
   const int tiles_per_img = p.tiles_y * p.tiles_x;
@@ -95,7 +88,6 @@ __device__ __forceinline__ void producer_flat(const ConvTcParams& p, const Ring&
   const uint32_t b_tile_bytes = (uint32_t)p.block_n * (uint32_t)bk * 2u;
   int st = 0;
   uint32_t phase = 0;
-  long long st_a = 0;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const int prob = tile / p.tiles_per_prob;
     const int t_in = tile - prob * p.tiles_per_prob;
@@ -111,9 +103,7 @@ __device__ __forceinline__ void producer_flat(const ConvTcParams& p, const Ring&
     int cc = 0, r = 0, sx = 0;
     for (int q0 = 0; q0 < T; q0 += G) {
       const int cnt = min(G, T - q0);
-      const long long t0 = STATS ? clock64() : 0;
       mbar_wait(rg.aempty(st), phase ^ 1);
-      if (STATS) st_a += clock64() - t0;
       const uint32_t a_slot = rg.a_base + st * rg.a_stage_bytes, b_slot = rg.b_base + st * rg.b_stage_bytes;
       if (elect_one()) mbar_expect_tx(rg.afull(st), (uint32_t)cnt * (a_box_bytes + b_tile_bytes));
       __syncwarp();
@@ -127,7 +117,6 @@ __device__ __forceinline__ void producer_flat(const ConvTcParams& p, const Ring&
       if (++st == stages) { st = 0; phase ^= 1; }
     }
   }
-  if (STATS && lane == 0) { p.stats[blockIdx.x * 8 + 0] = st_a; p.stats[blockIdx.x * 8 + 1] = 0; }
 }
 
 // ---------------------------------------------------------------- consumer warpgroups (MMA + epilogue)
@@ -284,14 +273,9 @@ conv_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
   if (warp == 0) {
-    const bool st = p.stats != nullptr;
-#define VPS_ROLE(FN, ...) \
-    do { if (st) FN<__VA_ARGS__, true>(p, rg, &tmA, &tmB0, &tmB1, &tmB2, &tmB3, lane); \
-         else FN<__VA_ARGS__, false>(p, rg, &tmA, &tmB0, &tmB1, &tmB2, &tmB3, lane); } while (0)
-    if (p.halo) { if (p.rowg) VPS_ROLE(producer_halo, true); else VPS_ROLE(producer_halo, false); }
-    else { if (st) producer_flat<true>(p, rg, &tmA, &tmB0, &tmB1, &tmB2, &tmB3, lane);
-           else producer_flat<false>(p, rg, &tmA, &tmB0, &tmB1, &tmB2, &tmB3, lane); }
-#undef VPS_ROLE
+    if (!p.halo) producer_flat(p, rg, &tmA, &tmB0, &tmB1, &tmB2, &tmB3);
+    else if (p.rowg) producer_halo<true>(p, rg, &tmA, &tmB0, &tmB1, &tmB2, &tmB3);
+    else producer_halo<false>(p, rg, &tmA, &tmB0, &tmB1, &tmB2, &tmB3);
   } else if (warp >= 4) {
     if (p.bk == 64) consumer_tc_n<true>(p, rg, (warp - 4) >> 2);
     else consumer_tc_n<false>(p, rg, (warp - 4) >> 2);
@@ -321,7 +305,6 @@ struct DcnParams {
 __device__ __forceinline__ void dcn_gather_loop(const ConvTcParams& p, const DcnParams& d, const Ring& rg, uint32_t setup_base,
                                                 int gtid) {
   const int stages = p.a_stages, cin_chunks = p.cin_chunks;
-  const int H = d.H, W = d.W;
   int st = 0;
   uint32_t phase = 0;
   const int j = gtid & 7;                    // 16-byte channel chunk of the 128-byte row
@@ -332,29 +315,7 @@ __device__ __forceinline__ void dcn_gather_loop(const ConvTcParams& p, const Dcn
     for (int item = gtid; item < 9 * BLOCK_M; item += 32 * DCN_GATHER_WARPS) {
       const int k = item >> 7, r = item & (BLOCK_M - 1);
       const int ty_in = r / p.tw, tx_in = r - ty_in * p.tw;
-      const int yo = ty * p.th + ty_in, xo = tx * p.tw + tx_in;
-      float wts[4] = {0.f, 0.f, 0.f, 0.f};
-      int offs[4] = {0, 0, 0, 0};
-      if (yo < H && xo < W) {
-        const float* op = d.off + ((int64_t)(img * H + yo) * W + xo) * d.off_cs;
-        const float oh = __ldg(op + 2 * k), ow = __ldg(op + 2 * k + 1);
-        const float h = (float)(yo - 1 + k / 3) + oh;
-        const float w = (float)(xo - 1 + k % 3) + ow;
-        if (h > -1.f && w > -1.f && h < (float)H && w < (float)W) {
-          const int hl = (int)floorf(h), wl = (int)floorf(w);
-          const int hh_ = hl + 1, wh_ = wl + 1;
-          const float lh = h - (float)hl, lw = w - (float)wl;
-          const float hh = 1.f - lh, hw = 1.f - lw;
-          const int base = img * H;
-          if (hl >= 0 && wl >= 0) { wts[0] = hh * hw; offs[0] = ((base + hl) * W + wl) * d.x_cs; }
-          if (hl >= 0 && wh_ <= W - 1) { wts[1] = hh * lw; offs[1] = ((base + hl) * W + wh_) * d.x_cs; }
-          if (hh_ <= H - 1 && wl >= 0) { wts[2] = lh * hw; offs[2] = ((base + hh_) * W + wl) * d.x_cs; }
-          if (hh_ <= H - 1 && wh_ <= W - 1) { wts[3] = lh * lw; offs[3] = ((base + hh_) * W + wh_) * d.x_cs; }
-        }
-      }
-      const uint32_t sa = setup_base + (uint32_t)item * 32u;
-      asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(sa), "f"(wts[0]), "f"(wts[1]), "f"(wts[2]), "f"(wts[3]) : "memory");
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sa + 16u), "r"(offs[0]), "r"(offs[1]), "r"(offs[2]), "r"(offs[3]) : "memory");
+      dcn_setup_entry(d, setup_base + (uint32_t)item * 32u, img, ty * p.th + ty_in, tx * p.tw + tx_in, k);
     }
     asm volatile("bar.sync 1, %0;" ::"n"(32 * DCN_GATHER_WARPS) : "memory");
     // ---- K steps: chunk-major, tap-minor
@@ -465,38 +426,9 @@ __global__ void pack_weights_tc_kernel(const float* __restrict__ src, const floa
                                        int cout_pad, int cin_pad, int transposed) {
   const int64_t total = (int64_t)cout_pad * kh * kw * cin_pad;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    const int ci = (int)(i % cin_pad);
-    int64_t t = i / cin_pad;
-    const int s = (int)(t % kw); t /= kw;
-    const int r = (int)(t % kh); t /= kh;
-    const int co = (int)t;
-    float v = 0.f;
-    if (co < cout && ci < cin) {
-      const int64_t si = transposed ? ((((int64_t)ci * cout + co) * kh + r) * kw + s)
-                                    : ((((int64_t)co * cin + ci) * kh + r) * kw + s);
-      v = src[si];
-      if (scale) v *= scale[co];
-    }
-    dst[i] = __float2bfloat16_rn(v);
-  }
+       i += (int64_t)gridDim.x * blockDim.x)
+    dst[i] = __float2bfloat16_rn(packed_weight(src, scale, i, cout, cin, kh, kw, cin_pad, transposed));
 }
-
-// ---------------------------------------------------------------- host
-PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = (PFN_cuTensorMapEncodeTiled_v12000)p;
-  }
-  return fn;
-}
-
-int g_num_sms = 0;
 
 }  // namespace
 
@@ -536,16 +468,12 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
                       args[i].cin_gran == a->cin_gran,
                   "conv2d_tc_multi: problems must share geometry");
   }
-  auto encode = get_encode();
-  if (!encode) { vps::set_error("cuTensorMapEncodeTiled unavailable"); return VPS_E_CUDA; }
-  if (!g_num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
-  }
+  auto encode = vps::tensor_map_encoder();
+  if (!encode) return VPS_E_CUDA;
+  const int sms = vps::num_sms();
+  if (sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
 
-  ConvTcParams p;
+  ConvTcParams p = {};
   const int bk = a->cin_gran == 16 ? 16 : 64;
   p.bk = bk;
   const int cin_pad = cin_pad_for(a->cin, bk);
@@ -553,28 +481,10 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
   p.n_img = a->x.n; p.oh = a->oh; p.ow = a->ow;
   // halo mode (stride 1, more than one tap): the 8 rows of an MMA row group are 8 consecutive pixels of one halo row,
   // so the tile is 16 x 8 pixels and every tap reads the same (16+kh-1) x (8+kw-1) box at a shifted start address.
-  static int halo_env = -1;
-  if (halo_env < 0) {
-    const char* e = getenv("VPS_CONV_HALO");
-    halo_env = e ? atoi(e) : 2;                         // 0 = off, 1 = on wherever legal, 2 = heuristic
-  }
-  const bool halo_ok = a->sh == 1 && a->sw == 1 && a->kh * a->kw > 1 && a->kh <= 8 && a->kw <= 8;
-  const bool halo = halo_ok && halo_env != 0;
+  const bool halo = a->sh == 1 && a->sw == 1 && a->kh * a->kw > 1 && a->kh <= 8 && a->kw <= 8;
   p.halo = halo ? 1 : 0;
-  if (halo) {
-    p.tw = 8; p.th = 16;
-  } else {
-    // pixel patch: minimise padded area; th*tw == 128, box extent tw*sw <= 256
-    int best_tw = 16; int64_t best_area = -1;
-    const int cands[5] = {16, 8, 32, 64, 128};
-    for (int i = 0; i < 5; ++i) {
-      const int tw = cands[i], th = 128 / tw;
-      if (tw * a->sw > 256 || th * a->sh > 256) continue;
-      const int64_t area = (int64_t)vps::cdiv(a->ow, tw) * tw * vps::cdiv(a->oh, th) * th;
-      if (best_area < 0 || area < best_area) { best_area = area; best_tw = tw; }
-    }
-    p.tw = best_tw; p.th = 128 / best_tw;
-  }
+  p.tw = halo ? 8 : patch_tw(a->oh, a->ow, BLOCK_M, a->sh, a->sw);
+  p.th = BLOCK_M / p.tw;
   p.halo_w = p.tw + a->kw - 1;
   const int halo_h = p.th + a->kh - 1;
   p.a_box_bytes = halo ? halo_h * p.halo_w * bk * 2 : BLOCK_M * bk * 2;
@@ -590,7 +500,7 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
     for (int bn = 16; bn <= 256 && bn <= cout_pad; bn *= 2) {     // the N extents the consumer is instantiated for
       if (cout_pad % bn) continue;
       const int64_t tiles = m_tiles * (cout_pad / bn);
-      const double waves = (double)((tiles + g_num_sms - 1) / g_num_sms);
+      const double waves = (double)((tiles + sms - 1) / sms);
       const double epi = 40.0 * bn;     // epilogue clocks per tile (not hidden when a CTA runs a single tile)
       double t;
       if (halo) {   // per tap: MMA time / operand reads from smem / weight box; per chunk: one halo box
@@ -635,43 +545,15 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
   p.nprob = nprob;
   p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
   p.total_tiles = p.tiles_per_prob * nprob;
-  p.y = a->y.ptr; p.y_h = a->y.h; p.y_w = a->y.w; p.y_cs = a->y.cs; p.y_dtype = a->y.dtype;
-  const int esz = a->y.dtype == VPS_BF16 ? 2 : 4;
-  p.y_vec = (((uintptr_t)a->y.ptr & 15) == 0) && ((a->y.cs * esz) % 16 == 0);
-  if (p.y_vec && (((uintptr_t)a->y.ptr & 31) == 0) && ((a->y.cs * esz) % 32 == 0)) p.y_vec = 2;     // 256-bit stores
-  p.oy_mul = a->oy_mul; p.ox_mul = a->ox_mul;
-  for (int i = 0; i < MAX_PROB; ++i) {
-    const vps_conv_args* q = &args[i < nprob ? i : 0];
-    p.ph_[i] = q->ph; p.pw_[i] = q->pw; p.oy_off_[i] = q->oy_off; p.ox_off_[i] = q->ox_off;
-    VPS_CHECK_ARG((a->oh - 1) * a->oy_mul + q->oy_off < a->y.h && (a->ow - 1) * a->ox_mul + q->ox_off < a->y.w,
-                  "conv2d_tc: output mapping out of range");
-  }
-  p.res = a->res.ptr; p.res_cs = a->res.cs; p.res_dtype = a->res.dtype; p.res_after_act = a->res_after_act;
-  p.res_vec = a->res.ptr && (((uintptr_t)a->res.ptr & 15) == 0) && (a->res.cs % 8 == 0);
-  if (p.res_vec && (((uintptr_t)a->res.ptr & 31) == 0) && (a->res.cs % 16 == 0)) p.res_vec = 2;       // 256-bit loads
-  VPS_CHECK_ARG(!a->bias || ((uintptr_t)a->bias & 15) == 0, "conv2d_tc: bias must be 16-byte aligned");
-  p.bias = a->bias; p.cout = a->cout; p.act = a->act; p.slope = a->slope; p.out_scale = a->out_scale;
-  if (a->res.ptr) VPS_CHECK_ARG(a->res.h == a->y.h && a->res.w == a->y.w, "conv2d_tc: residual geometry");
+  const int st = set_problems(p, args, nprob, "conv2d_tc");
+  if (st != VPS_OK) return st;
   if (p.total_tiles == 0) return VPS_OK;
 
   CUtensorMap tmA, tmB[MAX_PROB];
   const CUtensorMapSwizzle swz = bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_32B;
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)a->x.c, (cuuint64_t)a->x.w, (cuuint64_t)a->x.h, (cuuint64_t)a->x.n};
-    cuuint64_t strides[3] = {(cuuint64_t)a->x.cs * 2, (cuuint64_t)a->x.w * a->x.cs * 2,
-                             (cuuint64_t)a->x.h * a->x.w * a->x.cs * 2};
-    cuuint32_t box[4] = {(cuuint32_t)bk, (cuuint32_t)(halo ? p.halo_w : p.tw * a->sw),
-                         (cuuint32_t)(halo ? halo_h : p.th * a->sh), 1};
-    cuuint32_t estr[4] = {1, (cuuint32_t)a->sw, (cuuint32_t)a->sh, 1};
-    CUresult r = encode(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, a->x.ptr, dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      vps::set_error("conv2d_tc: encode A failed (%d) dims %d,%d,%d,%d cs %d box %d,%d,%d", (int)r, a->x.c,
-                     a->x.w, a->x.h, a->x.n, a->x.cs, bk, p.tw * a->sw, p.th * a->sh);
-      return VPS_E_CUDA;
-    }
-  }
+  if (!vps::encode_nhwc(&tmA, a->x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, bk, halo ? p.halo_w : p.tw * a->sw,
+                        halo ? halo_h : p.th * a->sh, a->sw, a->sh, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "conv2d_tc: encode A"))
+    return VPS_E_CUDA;
   for (int i = 0; i < MAX_PROB; ++i) {
     const vps_conv_args* q = &args[i < nprob ? i : 0];
     // packed weights [cout_pad][tap][cin_pad] viewed as {cin_pad, cout_pad, taps}: a box is {bk, block_n, taps-per-slot},
@@ -687,53 +569,8 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
     if (r != CUDA_SUCCESS) { vps::set_error("conv2d_tc: encode B failed (%d)", (int)r); return VPS_E_CUDA; }
   }
   const int smem = p.a_stages * p.a_stage_bytes + p.b_stages * b_stage_bytes + 1024 + 8 * (4 * MAX_STAGES + 8);
-  static bool smem_set = false;
-  if (!smem_set) {
-    if (cudaFuncSetAttribute(conv_igemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) !=
-        cudaSuccess) {
-      vps::set_error("conv2d_tc: cannot raise dynamic smem: %s", cudaGetErrorString(cudaGetLastError()));
-      return VPS_E_CUDA;
-    }
-    smem_set = true;
-  }
-  const int grid = p.total_tiles < g_num_sms ? p.total_tiles : g_num_sms;
-  static int stats_env = -1;
-  static long long* stats_buf = nullptr;
-  if (stats_env < 0) { const char* e = getenv("VPS_CONV_STATS"); stats_env = e ? atoi(e) : 0; }
-  p.stats = nullptr;
-  if (stats_env) {   // debugging aid: per-role barrier-wait clocks, printed after a device sync (never on in production)
-    if (!stats_buf) cudaMalloc(&stats_buf, sizeof(long long) * 8 * 1024);
-    cudaMemsetAsync(stats_buf, 0, sizeof(long long) * 8 * grid, (cudaStream_t)stream);
-    p.stats = stats_buf;
-  }
-  static int pdl_env = -1;
-  if (pdl_env < 0) { const char* e = getenv("VPS_PDL"); pdl_env = e ? atoi(e) : 1; }
-  {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(NUM_THREADS); cfg.dynamicSmemBytes = (size_t)smem;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_env ? 1 : 0;
-    const cudaError_t le = cudaLaunchKernelEx(&cfg, conv_igemm_tc_kernel, tmA, tmB[0], tmB[1], tmB[2], tmB[3], p);
-    if (le != cudaSuccess) { vps::set_error("conv2d_tc: launch failed: %s", cudaGetErrorString(le)); return VPS_E_CUDA; }
-  }
-  VPS_CUDA_LAST("conv_igemm_tc_kernel");
-  if (stats_env) {
-    static long long h[8 * 1024];
-    cudaStreamSynchronize((cudaStream_t)stream);
-    cudaMemcpy(h, stats_buf, sizeof(long long) * 8 * grid, cudaMemcpyDeviceToHost);
-    double m[8] = {0};
-    for (int i = 0; i < grid; ++i) for (int j = 0; j < 8; ++j) m[j] += (double)h[i * 8 + j] / grid;
-    const int tiles_cta = (p.total_tiles + grid - 1) / grid;
-    // slots 0 / 1: the producer's clocks waiting for free A / B ring slots (the only role that records them)
-    fprintf(stderr, "conv_tc stats %dx%d %d->%d @%dx%d halo=%d/%d g%d bn=%d bk=%d stages a%d b%d tiles/cta %d steps/tile %d | clk/CTA: "
-            "prod wait Aempty %.0f Bempty %.0f\n",
-            a->kh, a->kw, a->cin, a->cout, a->oh, a->ow, p.halo, p.rowg, p.gsub, block_n, bk, p.a_stages, p.b_stages, tiles_cta,
-            a->kh * a->kw * p.cin_chunks, m[0], m[1]);
-  }
-  return VPS_OK;
+  return launch_persistent<conv_igemm_tc_kernel>(p.total_tiles, NUM_THREADS, smem, stream, "conv2d_tc", tmA, tmB[0], tmB[1],
+                                                 tmB[2], tmB[3], p);
 }
 
 extern "C" int vps_conv2d_tc(const vps_conv_args* a, void* stream) { return vps_conv2d_tc_multi(a, 1, stream); }
@@ -751,30 +588,18 @@ extern "C" int vps_deform_conv_tc(const vps_tensor* x, const vps_tensor* offset,
   VPS_CHECK_ARG((int64_t)x->n * x->h * x->w * x->cs < (1ll << 31), "deform_conv_tc: tensor too large for 32-bit offsets");
   const int cout_pad = (cout + 15) / 16 * 16;
   VPS_CHECK_ARG(cout_pad <= 256 && ((uintptr_t)w & 15) == 0, "deform_conv_tc: cout %d > 256", cout);
-  auto encode = get_encode();
-  if (!encode) { vps::set_error("cuTensorMapEncodeTiled unavailable"); return VPS_E_CUDA; }
-  if (!g_num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
-  }
+  auto encode = vps::tensor_map_encoder();
+  if (!encode) return VPS_E_CUDA;
+  if (vps::num_sms() <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
   ConvTcParams p = {};
   p.bk = 64; p.nprob = 1;
   p.n_img = x->n; p.oh = x->h; p.ow = x->w;
-  int best_tw = 16; int64_t best_area = -1;
-  const int cands[5] = {16, 8, 32, 64, 128};
-  for (int i = 0; i < 5; ++i) {
-    const int tw = cands[i], th = 128 / tw;
-    const int64_t area = (int64_t)vps::cdiv(x->w, tw) * tw * vps::cdiv(x->h, th) * th;
-    if (best_area < 0 || area < best_area) { best_area = area; best_tw = tw; }
-  }
-  p.tw = best_tw; p.th = 128 / best_tw;
+  p.tw = patch_tw(x->h, x->w, BLOCK_M, 1, 1); p.th = BLOCK_M / p.tw;
   p.tiles_x = vps::cdiv(x->w, p.tw); p.tiles_y = vps::cdiv(x->h, p.th);
   // weight rows past cout_pad are TMA zero fill
   p.block_n = cout_pad <= 64 ? 64 : DCN_MAX_N;
   p.n_tiles_n = vps::cdiv(cout_pad, p.block_n);
-  p.kh = p.kw = 3; p.sh = p.sw = 1; p.ph = p.pw = 1;
+  p.kh = p.kw = 3; p.sh = p.sw = 1;
   p.cin_chunks = x->c / 64;
   p.gsub = 1; p.nk_last = 4; p.halo = 0; p.rowg = 0;
   p.a_box_bytes = BLOCK_M * 128; p.a_stage_bytes = p.a_box_bytes;
@@ -785,13 +610,9 @@ extern "C" int vps_deform_conv_tc(const vps_tensor* x, const vps_tensor* offset,
   p.a_stages = p.b_stages = stages;
   p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
   p.total_tiles = p.tiles_per_prob;
-  p.y = y->ptr; p.y_h = y->h; p.y_w = y->w; p.y_cs = y->cs; p.y_dtype = y->dtype;
-  const int esz = y->dtype == VPS_BF16 ? 2 : 4;
-  p.y_vec = (((uintptr_t)y->ptr & 15) == 0) && ((y->cs * esz) % 16 == 0);
-  if (p.y_vec && (((uintptr_t)y->ptr & 31) == 0) && ((y->cs * esz) % 32 == 0)) p.y_vec = 2;
+  set_output(p, *y);
   p.oy_mul = p.ox_mul = 1;
-  p.res = nullptr; p.bias = nullptr; p.cout = cout; p.act = VPS_ACT_NONE; p.slope = 0.f; p.out_scale = 1.f;
-  p.stats = nullptr;
+  p.cout = cout; p.act = VPS_ACT_NONE; p.out_scale = 1.f;
   if (p.total_tiles == 0) return VPS_OK;
   DcnParams d;
   d.x = (const __nv_bfloat16*)x->ptr; d.off = (const float*)offset->ptr; d.x_cs = x->cs; d.off_cs = offset->cs;
@@ -808,24 +629,5 @@ extern "C" int vps_deform_conv_tc(const vps_tensor* x, const vps_tensor* offset,
     if (r != CUDA_SUCCESS) { vps::set_error("deform_conv_tc: encode B failed (%d)", (int)r); return VPS_E_CUDA; }
   }
   const int smem = stages * stage_bytes + DCN_SETUP_BYTES + 1024 + 8 * (4 * MAX_STAGES + 8);
-  static bool smem_set = false;
-  if (!smem_set) {
-    if (cudaFuncSetAttribute(dcn_igemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
-      vps::set_error("deform_conv_tc: cannot raise dynamic smem: %s", cudaGetErrorString(cudaGetLastError()));
-      return VPS_E_CUDA;
-    }
-    smem_set = true;
-  }
-  const int grid = p.total_tiles < g_num_sms ? p.total_tiles : g_num_sms;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(DCN_THREADS); cfg.dynamicSmemBytes = (size_t)smem;
-  cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  const cudaError_t le = cudaLaunchKernelEx(&cfg, dcn_igemm_tc_kernel, tmB, p, d);
-  if (le != cudaSuccess) { vps::set_error("deform_conv_tc: launch failed: %s", cudaGetErrorString(le)); return VPS_E_CUDA; }
-  VPS_CUDA_LAST("dcn_igemm_tc_kernel");
-  return VPS_OK;
+  return launch_persistent<dcn_igemm_tc_kernel>(p.total_tiles, DCN_THREADS, smem, stream, "deform_conv_tc", tmB, p, d);
 }

@@ -37,8 +37,6 @@
 // (the promotion order above), so a warpgroup spends a fixed few hundred clocks per step whatever N is; at N <= 64 four
 // warpgroups overlap those round trips and share each converted box and weight tile among twice the pixels.  At 640
 // threads the register cap is 96, which holds the N = 64 step accumulator + sum.  vps_conv2d_tc32_plan picks NWG.
-#include <cuda_fp16.h>
-
 #include "conv_tc_common.cuh"
 
 namespace {
@@ -51,7 +49,6 @@ constexpr int T32_WIDE_MAX_N = 64;          // NWG = 4: 2 x 32 registers at N = 
 constexpr int t32_threads(int nwg) { return 128 * (nwg + 1); }
 constexpr int T32_STAGE_SLOTS = 2;          // fp32 staging boxes (TMA -> converters)
 constexpr int T32_PLANES = 2;               // operand planes: fp16(v), fp16(2^11 (v - fp16(v)))
-constexpr float T32_LO_SCALE = 2048.f, T32_LO_INV = 1.f / 2048.f;
 
 __device__ unsigned int g_tc32_overflow = 0;     // activations / weights that exceeded the fp16 range of the main product
 
@@ -60,10 +57,8 @@ struct Tc32Extra {
   int plane_bytes;           // bytes of one operand plane of an A item (rows * 64, padded to 1024)
   int stage_bytes;           // bytes of one fp32 staging slot (rows * 128, padded to 1024)
   int b_plane_bytes;         // block_n * 64: one weight plane of one step
-  int nk_last;               // K16 slabs of the last channel chunk that hold real channels
   int dcn;                   // 1: the operand planes are produced by the deformable-sampling warps (no activation TMA)
   int dcn_split_n;           // DCN split-N layout: the consumer warpgroups share the tile's pixels, each takes block_n / 2 channels
-  int sleep_ns;              // back-off of the converter / producer waits (VPS_TC32_SLEEP, default 0 = poll)
 };
 
 struct Dcn32Params {
@@ -114,54 +109,6 @@ constexpr int t32_box_c(int n) { return n >= 32 ? 32 : 16; }
 constexpr int T32_EPI_MAX_N = 64;
 constexpr int t32_epi_bytes(int nwg, int bn) { return 64 * nwg * bn * 4 + nwg * bn * 4; }    // output boxes + bias
 
-__device__ __forceinline__ void tma_load_5d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, int c3,
-                                            int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4, %5, %6, %7}], [%2];" ::"r"(dst),
-      "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-// shared -> global tensor store of one box (clipped at the tensor bounds), in the issuing thread's bulk async-group
-__device__ __forceinline__ void tma_store_4d(const void* tmap, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(tmap), "r"(src),
-               "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-// fp16 (round to nearest, saturating) of v; `over` collects |v| > 65504 (and NaN)
-__device__ __forceinline__ float to_f16_sat(float v, unsigned short& bits, bool& over) {
-  unsigned short h;
-  asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(v));
-  bits = h;
-  over = over || !(fabsf(v) <= 65504.f);
-  return __half2float(__ushort_as_half(h));
-}
-
-// operand split of two values at once: hi = packed fp16x2 of (v0, v1) (round to nearest, saturating), lo = packed fp16x2 of
-// 2^11 * (v - fp16(v)).  Same values as two to_f16_sat() pairs with 10 instead of 14 instructions (the converter and the
-// deformable sampler are bound by exactly this arithmetic).
-__device__ __forceinline__ void split_pair_f16(float v0, float v1, uint32_t& hi, uint32_t& lo, bool& over) {
-  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(v1), "f"(v0));       // first source -> upper half
-  over = over || !(fabsf(v0) <= 65504.f) || !(fabsf(v1) <= 65504.f);
-  const float2 h = __half22float2(*reinterpret_cast<const __half2*>(&hi));
-  const float r0 = (v0 - h.x) * T32_LO_SCALE, r1 = (v1 - h.y) * T32_LO_SCALE;          // exact in fp32
-  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(r1), "f"(r0));
-}
-
-// wait with back-off for roles with slack (converters, TMA producer): a failed poll sleeps instead of re-polling at once, so
-// that the idle warps' polling does not queue in front of the latency-critical issuers' shared-memory / barrier operations
-__device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity, uint32_t ns) {
-  uint32_t done = 0, spins = 0;
-  while (true) {
-    asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
-                 : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (done) break;
-    if (ns) __nanosleep(ns);
-    if (++spins > (1u << VPS_MBAR_SPIN_LOG2)) __trap();      // a lost arrival fails loudly (no printf: a call in the kernel
-                                                               // makes ptxas serialise the consumers' wgmma pipeline)
-  }
-}
-
 // ---------------------------------------------------------------- warp 0: TMA producer
 __device__ __forceinline__ void producer32(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, const CUtensorMap* tmA,
                                            const CUtensorMap* tmB) {
@@ -180,7 +127,7 @@ __device__ __forceinline__ void producer32(const ConvTcParams& p, const Tc32Extr
       int r = 0, s = 0;
       for (int tap = 0; tap < ntaps; ++tap) {
         if (!e.dcn && (!halo || tap == 0)) {
-          mbar_wait_relaxed(rg.sempty(ss), sphase ^ 1, (uint32_t)e.sleep_ns);
+          mbar_wait(rg.sempty(ss), sphase ^ 1);
           if (elect_one()) {
             mbar_expect_tx(rg.sfull(ss), a_box_bytes);
             tma_load_4d(rg.s_base + ss * rg.s_bytes, tmA, rg.sfull(ss), cc * T32_KC, halo ? x_base : x_base + s,
@@ -188,7 +135,7 @@ __device__ __forceinline__ void producer32(const ConvTcParams& p, const Tc32Extr
           }
           if (++ss == T32_STAGE_SLOTS) { ss = 0; sphase ^= 1; }
         }
-        mbar_wait_relaxed(rg.bempty(bs), bphase ^ 1, (uint32_t)e.sleep_ns);
+        mbar_wait(rg.bempty(bs), bphase ^ 1);
         if (elect_one()) {     // both weight planes of this (tap, chunk) in one 5-D box
           mbar_expect_tx(rg.bfull(bs), b_bytes);
           tma_load_5d(rg.b_base + bs * rg.b_bytes, tmB, rg.bfull(bs), cc * T32_KC, n0, tap, t.prob, 0);
@@ -210,8 +157,8 @@ __device__ __forceinline__ void converter32(const ConvTcParams& p, const Tc32Ext
   bool over = false;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     for (int it = 0; it < items_per_tile; ++it) {
-      mbar_wait_relaxed(rg.sfull(ss), sphase, (uint32_t)e.sleep_ns);
-      mbar_wait_relaxed(rg.pempty(as), aphase ^ 1, (uint32_t)e.sleep_ns);
+      mbar_wait(rg.sfull(ss), sphase);
+      mbar_wait(rg.pempty(as), aphase ^ 1);
       const uint32_t src = rg.s_base + ss * rg.s_bytes;
       const uint32_t dst = rg.a_base + as * rg.a_bytes;
       for (int task = ctid; task < tasks; task += nthreads) {
@@ -254,7 +201,6 @@ __device__ __forceinline__ void converter32(const ConvTcParams& p, const Tc32Ext
 __device__ __forceinline__ void dcn_gather32(const ConvTcParams& p, const Tc32Extra& e, const Dcn32Params& d, const Ring32& rg,
                                              uint32_t setup_base, uint32_t ctr_addr, int gtid) {
   constexpr int NT = 32 * DCN32_GATHER_WARPS;
-  const int H = d.H, W = d.W;
   const int lane = gtid & 31;
   const int j = lane & 3;                    // 8-channel group of the 32-channel chunk
   const int rlog = e.rows == 128 ? 7 : 6, ulog = rlog - 3;
@@ -269,29 +215,7 @@ __device__ __forceinline__ void dcn_gather32(const ConvTcParams& p, const Tc32Ex
     for (int item = gtid; item < 9 << rlog; item += NT) {
       const int k = item >> rlog, r = item & ((1 << rlog) - 1);
       const int ty_in = r / p.tw, tx_in = r - ty_in * p.tw;
-      const int yo = t.ty * p.th + ty_in, xo = t.tx * p.tw + tx_in;
-      float wts[4] = {0.f, 0.f, 0.f, 0.f};
-      int offs[4] = {0, 0, 0, 0};
-      if (yo < H && xo < W) {
-        const float* op = d.off + ((int64_t)(t.img * H + yo) * W + xo) * d.off_cs;
-        const float oh = __ldg(op + 2 * k), ow = __ldg(op + 2 * k + 1);
-        const float h = (float)(yo - 1 + k / 3) + oh;
-        const float w = (float)(xo - 1 + k % 3) + ow;
-        if (h > -1.f && w > -1.f && h < (float)H && w < (float)W) {
-          const int hl = (int)floorf(h), wl = (int)floorf(w);
-          const int hh_ = hl + 1, wh_ = wl + 1;
-          const float lh = h - (float)hl, lw = w - (float)wl;
-          const float hh = 1.f - lh, hw = 1.f - lw;
-          const int base = t.img * H;
-          if (hl >= 0 && wl >= 0) { wts[0] = hh * hw; offs[0] = ((base + hl) * W + wl) * d.x_cs; }
-          if (hl >= 0 && wh_ <= W - 1) { wts[1] = hh * lw; offs[1] = ((base + hl) * W + wh_) * d.x_cs; }
-          if (hh_ <= H - 1 && wl >= 0) { wts[2] = lh * hw; offs[2] = ((base + hh_) * W + wl) * d.x_cs; }
-          if (hh_ <= H - 1 && wh_ <= W - 1) { wts[3] = lh * lw; offs[3] = ((base + hh_) * W + wh_) * d.x_cs; }
-        }
-      }
-      const uint32_t sa = setup_base + (uint32_t)item * 32u;
-      asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(sa), "f"(wts[0]), "f"(wts[1]), "f"(wts[2]), "f"(wts[3]) : "memory");
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sa + 16u), "r"(offs[0]), "r"(offs[1]), "r"(offs[2]), "r"(offs[3]) : "memory");
+      dcn_setup_entry(d, setup_base + (uint32_t)item * 32u, t.img, t.ty * p.th + ty_in, t.tx * p.tw + tx_in, k);
     }
     asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory");
     // ---- units are claimed dynamically (any number of gather warps stays balanced; a warp may run ahead into the next
@@ -447,7 +371,7 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
 #pragma unroll
     for (int i = 0; i < N / 2; ++i) sum[i] = 0.f;
     for (int cc = 0; cc <= last_cc; ++cc) {
-      const bool two = cc != last_cc || e.nk_last > 1;
+      const bool two = cc != last_cc || p.nk_last > 1;
       uint32_t a_item = 0;
       int r = 0, s = 0;
       for (int tap = 0; tap < ntaps; ++tap) {
@@ -616,53 +540,19 @@ __global__ void pack_weights_tc32_kernel(const float* __restrict__ src, const fl
   const int64_t total = (int64_t)cout_pad * kh * kw * cin_pad;
   bool over = false;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const int ci = (int)(i % cin_pad);
-    int64_t t = i / cin_pad;
-    const int s = (int)(t % kw); t /= kw;
-    const int r = (int)(t % kh); t /= kh;
-    const int co = (int)t;
-    float v = 0.f;
-    if (co < cout && ci < cin) {
-      const int64_t si = transposed ? ((((int64_t)ci * cout + co) * kh + r) * kw + s) : ((((int64_t)co * cin + ci) * kh + r) * kw + s);
-      v = src[si];
-      if (scale) v *= scale[co];
-    }
+    const float v = packed_weight(src, scale, i, cout, cin, kh, kw, cin_pad, transposed);
     unsigned short h, l;
-    const float m = to_f16_sat(v, h, over);
-    bool dummy = false;
-    to_f16_sat((v - m) * T32_LO_SCALE, l, dummy);
+    split_f16(v, h, l);
+    over = over || f16_over(v);
     bm[i] = h;
     bl[i] = l;
   }
   if (over) atomicAdd(&g_tc32_overflow, 1u);
 }
 
-PFN_cuTensorMapEncodeTiled_v12000 get_encode32() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = (PFN_cuTensorMapEncodeTiled_v12000)p;
-  }
-  return fn;
-}
-int g_num_sms32 = 0;
-
 inline int64_t plane_elems(int cout, int cin, int kh, int kw) {
   const int64_t cout_pad = (cout + 15) / 16 * 16, cin_pad = (cin + T32_KC - 1) / T32_KC * T32_KC;
   return cout_pad * kh * kw * cin_pad;
-}
-
-int num_sms32() {
-  if (!g_num_sms32) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms32, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return g_num_sms32;
 }
 
 constexpr int T32_SMEM_BUDGET = 227 * 1024 - 1024 - T32_BAR_BYTES - 64;
@@ -695,19 +585,9 @@ Tc32Plan tc32_tile(const vps_conv_args* a, int nwg) {
   g.nwg = nwg;
   const int px = 64 * nwg;
   g.halo = a->sh == 1 && a->sw == 1 && a->kh * a->kw > 1 && a->kh <= 8 && a->kw <= 8;
-  if (g.halo) {          // 8-pixel halo rows: the consumer's descriptors step one halo row per 8-row group
-    g.tw = 8; g.th = px / 8;
-  } else {
-    int best_tw = 16; int64_t best_area = -1;
-    const int cands[6] = {16, 8, 32, 64, 128, 256};
-    for (int i = 0; i < 6; ++i) {
-      const int tw = cands[i], th = px / tw;
-      if (th == 0 || tw * a->sw > 256 || th * a->sh > 256) continue;     // TMA box extents
-      const int64_t area = (int64_t)vps::cdiv(a->ow, tw) * tw * vps::cdiv(a->oh, th) * th;
-      if (best_area < 0 || area < best_area) { best_area = area; best_tw = tw; }
-    }
-    g.tw = best_tw; g.th = px / best_tw;
-  }
+  // 8-pixel halo rows: the consumer's descriptors step one halo row per 8-row group
+  g.tw = g.halo ? 8 : patch_tw(a->oh, a->ow, px, a->sh, a->sw);
+  g.th = px / g.tw;
   g.halo_w = g.tw + a->kw - 1;
   g.halo_h = g.th + a->kh - 1;
   g.rows = g.halo ? g.halo_h * g.halo_w : px;
@@ -734,7 +614,7 @@ int tc32_plan(const vps_conv_args* a, int nprob, Tc32Plan& out) {
   VPS_CHECK_ARG(a->sh >= 1 && a->sh <= 2 && a->sw >= 1 && a->sw <= 2, "conv2d_tc32: stride must be 1 or 2");
   VPS_CHECK_ARG(a->kh >= 1 && a->kw >= 1 && a->cin >= 1 && a->cout >= 1 && a->oh >= 0 && a->ow >= 0 && a->x.n >= 0,
                 "conv2d_tc32: bad geometry (k %dx%d, cin %d, cout %d, out %dx%d)", a->kh, a->kw, a->cin, a->cout, a->oh, a->ow);
-  const int sms = num_sms32();
+  const int sms = vps::num_sms();
   if (sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
   const int cout_pad = (a->cout + 15) / 16 * 16;
   const int steps = (a->cin + T32_KC - 1) / T32_KC * a->kh * a->kw;
@@ -806,21 +686,14 @@ constexpr double DCN32_UNIT_CLK = 220.0, DCN32_STEP_CLK = 300.0;
 // Every N tile samples the same input again, so a tile as wide as cout_pad samples each input once; narrower tiles win where
 // the grid would otherwise leave SMs idle.  Equal costs go to the plan that samples less.
 int dcn32_plan(int n, int h, int w, int cin, int cout, Dcn32Plan& out) {
-  const int sms = num_sms32();
+  const int sms = vps::num_sms();
   if (sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
   const int cout_pad = (cout + 15) / 16 * 16;
   const int steps = cin / T32_KC * 9;
   double best = -1.0, best_units = 0.0;
   for (int split_n = 0; split_n <= 1; ++split_n) {
     const int rows = split_n ? 64 : 128;
-    int best_tw = 16; int64_t best_area = -1;
-    const int cands[5] = {16, 8, 32, 64, 128};
-    for (int i = 0; i < 5; ++i) {
-      const int tw = cands[i], th = rows / tw;
-      if (th == 0) continue;
-      const int64_t area = (int64_t)vps::cdiv(w, tw) * tw * vps::cdiv(h, th) * th;
-      if (best_area < 0 || area < best_area) { best_area = area; best_tw = tw; }
-    }
+    const int best_tw = patch_tw(h, w, rows, 1, 1);
     const int64_t m_tiles = (int64_t)n * vps::cdiv(h, rows / best_tw) * vps::cdiv(w, best_tw);
     const int a_side = 2 * T32_PLANES * rows * 64 + dcn32_setup_bytes(rows);
     for (int bn = 16; bn <= DCN32_MAX_N; bn *= 2) {
@@ -903,10 +776,10 @@ extern "C" int vps_conv2d_tc32_multi(const vps_conv_args* args, int nprob, void*
                       args[i].bias == a->bias && args[i].act == a->act && args[i].oy_mul == a->oy_mul && args[i].ox_mul == a->ox_mul,
                   "conv2d_tc32_multi: problems must share geometry and the packed weight buffer");
   }
-  auto encode = get_encode32();
-  if (!encode) { vps::set_error("cuTensorMapEncodeTiled unavailable"); return VPS_E_CUDA; }
+  auto encode = vps::tensor_map_encoder();
+  if (!encode) return VPS_E_CUDA;
   Tc32Plan g;
-  const int st = tc32_plan(a, nprob, g);
+  int st = tc32_plan(a, nprob, g);
   if (st != VPS_OK) return st;
   VPS_CHECK_ARG(g.b_stages >= 2, "conv2d_tc32: ring does not fit (%d x %d px halo, bn %d)", g.halo_h, g.halo_w, g.block_n);
   ConvTcParams p = {};
@@ -929,50 +802,25 @@ extern "C" int vps_conv2d_tc32_multi(const vps_conv_args* args, int nprob, void*
   p.kh = a->kh; p.kw = a->kw; p.sh = a->sh; p.sw = a->sw;
   p.cin_chunks = cin_pad / T32_KC;
   const int rem = a->cin - (p.cin_chunks - 1) * T32_KC;
-  e.nk_last = (rem + 15) / 16;
+  p.nk_last = (rem + 15) / 16;
   const int ntaps = a->kh * a->kw;
   p.a_stages = g.a_stages;
   const int block_n = g.block_n;
   p.block_n = block_n; p.n_tiles_n = cout_pad / block_n;
   e.b_plane_bytes = block_n * 64;
   p.b_stages = g.b_stages;
-  { static int sl_env = -1; if (sl_env < 0) { const char* ev = getenv("VPS_TC32_SLEEP"); sl_env = ev ? atoi(ev) : 0; } e.sleep_ns = sl_env; }
   p.nprob = nprob;
   p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
   p.total_tiles = p.tiles_per_prob * nprob;
-  p.y = a->y.ptr; p.y_h = a->y.h; p.y_w = a->y.w; p.y_cs = a->y.cs; p.y_dtype = a->y.dtype;
-  const int esz = a->y.dtype == VPS_BF16 ? 2 : 4;
-  p.y_vec = (((uintptr_t)a->y.ptr & 15) == 0) && ((a->y.cs * esz) % 16 == 0);
-  if (p.y_vec && (((uintptr_t)a->y.ptr & 31) == 0) && ((a->y.cs * esz) % 32 == 0)) p.y_vec = 2;
-  p.oy_mul = a->oy_mul; p.ox_mul = a->ox_mul;
-  for (int i = 0; i < MAX_PROB; ++i) {
-    const vps_conv_args* q = &args[i < nprob ? i : 0];
-    p.ph_[i] = q->ph; p.pw_[i] = q->pw; p.oy_off_[i] = q->oy_off; p.ox_off_[i] = q->ox_off;
-    VPS_CHECK_ARG((a->oh - 1) * a->oy_mul + q->oy_off < a->y.h && (a->ow - 1) * a->ox_mul + q->ox_off < a->y.w,
-                  "conv2d_tc32: output mapping out of range");
-  }
-  p.res = a->res.ptr; p.res_cs = a->res.cs; p.res_dtype = a->res.dtype; p.res_after_act = a->res_after_act;
-  p.res_vec = a->res.ptr && (((uintptr_t)a->res.ptr & 15) == 0) && (a->res.cs % 8 == 0);
-  if (p.res_vec && (((uintptr_t)a->res.ptr & 31) == 0) && (a->res.cs % 16 == 0)) p.res_vec = 2;
-  VPS_CHECK_ARG(!a->bias || ((uintptr_t)a->bias & 15) == 0, "conv2d_tc32: bias must be 16-byte aligned");
-  p.bias = a->bias; p.cout = a->cout; p.act = a->act; p.slope = a->slope; p.out_scale = a->out_scale;
-  if (a->res.ptr) VPS_CHECK_ARG(a->res.h == a->y.h && a->res.w == a->y.w, "conv2d_tc32: residual geometry");
-  p.stats = nullptr;
+  st = set_problems(p, args, nprob, "conv2d_tc32");
+  if (st != VPS_OK) return st;
   if (p.total_tiles == 0) return VPS_OK;
 
   CUtensorMap tmA, tmB;
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)a->x.c, (cuuint64_t)a->x.w, (cuuint64_t)a->x.h, (cuuint64_t)a->x.n};
-    cuuint64_t strides[3] = {(cuuint64_t)a->x.cs * 4, (cuuint64_t)a->x.w * a->x.cs * 4, (cuuint64_t)a->x.h * a->x.w * a->x.cs * 4};
-    cuuint32_t box[4] = {(cuuint32_t)T32_KC, (cuuint32_t)(halo ? p.halo_w : p.tw * a->sw), (cuuint32_t)(halo ? halo_h : p.th * a->sh), 1};
-    cuuint32_t estr[4] = {1, (cuuint32_t)a->sw, (cuuint32_t)a->sh, 1};
-    CUresult r = encode(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, a->x.ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      vps::set_error("conv2d_tc32: encode A failed (%d) dims %d,%d,%d,%d cs %d", (int)r, a->x.c, a->x.w, a->x.h, a->x.n, a->x.cs);
-      return VPS_E_CUDA;
-    }
-  }
+  if (!vps::encode_nhwc(&tmA, a->x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, T32_KC, halo ? p.halo_w : p.tw * a->sw,
+                        halo ? halo_h : p.th * a->sh, a->sw, a->sh, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                        "conv2d_tc32: encode A"))
+    return VPS_E_CUDA;
   const int64_t n_plane = (int64_t)cout_pad * ntaps * cin_pad;
   {
     cuuint64_t dims[5] = {(cuuint64_t)cin_pad, (cuuint64_t)cout_pad, (cuuint64_t)ntaps, (cuuint64_t)nprob, T32_PLANES};
@@ -991,44 +839,23 @@ extern "C" int vps_conv2d_tc32_multi(const vps_conv_args* args, int nprob, void*
     const int bc = t32_box_c(block_n), box_w = p.tw < 64 ? p.tw : 64;
     const int64_t px = (int64_t)a->oy_off * a->y.w + a->ox_off;
     for (int m = 0; m < (a->res.ptr ? 2 : 1); ++m) {
-      const vps_tensor& t = m ? a->res : a->y;
-      cuuint64_t dims[4] = {(cuuint64_t)a->cout, (cuuint64_t)a->ow, (cuuint64_t)a->oh, (cuuint64_t)a->x.n};
-      cuuint64_t strides[3] = {(cuuint64_t)t.cs * 4, (cuuint64_t)a->y.w * t.cs * 4, (cuuint64_t)a->y.h * a->y.w * t.cs * 4};
-      cuuint32_t box[4] = {(cuuint32_t)bc, (cuuint32_t)box_w, (cuuint32_t)(64 / box_w), 1};
-      cuuint32_t estr[4] = {1, 1, 1, 1};
-      CUresult r = encode(m ? &tmR : &tmY, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (float*)t.ptr + px * t.cs, dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, bc == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) { vps::set_error("conv2d_tc32: encode %s failed (%d)", m ? "residual" : "output", (int)r); return VPS_E_CUDA; }
+      const vps_tensor& t = m ? a->res : a->y;          // the residual has the output's geometry
+      vps_tensor v = t;
+      v.ptr = (float*)t.ptr + px * t.cs; v.n = a->x.n; v.h = a->oh; v.w = a->ow; v.c = a->cout;
+      if (!vps::encode_nhwc(m ? &tmR : &tmY, v, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, bc, box_w, 64 / box_w, 1, 1,
+                            bc == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                            m ? "conv2d_tc32: encode residual" : "conv2d_tc32: encode output", &t))
+        return VPS_E_CUDA;
     }
   }
   const int smem = g.a_side + p.b_stages * T32_PLANES * e.b_plane_bytes + (g.epi_tma ? t32_epi_bytes(g.nwg, block_n) : 0) + 1024 +
                    T32_BAR_BYTES;
-  const auto kernel = g.nwg == 4 ? (g.epi_tma ? conv_igemm_tc32_kernel<4, true> : conv_igemm_tc32_kernel<4, false>)
-                                  : (g.epi_tma ? conv_igemm_tc32_kernel<2, true> : conv_igemm_tc32_kernel<2, false>);
-  static bool smem_set[4] = {false, false, false, false};
-  const int inst = 2 * (g.nwg == 4) + g.epi_tma;
-  if (!smem_set[inst]) {
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
-      vps::set_error("conv2d_tc32: cannot raise dynamic smem: %s", cudaGetErrorString(cudaGetLastError()));
-      return VPS_E_CUDA;
-    }
-    smem_set[inst] = true;
-  }
-  const int grid = p.total_tiles < g_num_sms32 ? p.total_tiles : g_num_sms32;
-  static int pdl_env = -1;
-  if (pdl_env < 0) { const char* ev = getenv("VPS_PDL"); pdl_env = ev ? atoi(ev) : 1; }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(t32_threads(g.nwg)); cfg.dynamicSmemBytes = (size_t)smem;
-  cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_env ? 1 : 0;
-  const cudaError_t le = cudaLaunchKernelEx(&cfg, kernel, tmA, tmB, tmY, tmR, p, e);
-  if (le != cudaSuccess) { vps::set_error("conv2d_tc32: launch failed: %s", cudaGetErrorString(le)); return VPS_E_CUDA; }
-  VPS_CUDA_LAST("conv_igemm_tc32_kernel");
-  return VPS_OK;
+#define VPS_TC32_LAUNCH(NWG, EPI)                                                                                              \
+  launch_persistent<conv_igemm_tc32_kernel<NWG, EPI>>(p.total_tiles, t32_threads(NWG), smem, stream, "conv2d_tc32", tmA, tmB, tmY, \
+                                                      tmR, p, e)
+  if (g.nwg == 4) return g.epi_tma ? VPS_TC32_LAUNCH(4, true) : VPS_TC32_LAUNCH(4, false);
+  return g.epi_tma ? VPS_TC32_LAUNCH(2, true) : VPS_TC32_LAUNCH(2, false);
+#undef VPS_TC32_LAUNCH
 }
 
 extern "C" int vps_conv2d_tc32(const vps_conv_args* a, void* stream) { return vps_conv2d_tc32_multi(a, 1, stream); }
@@ -1054,8 +881,8 @@ extern "C" int vps_deform_conv_tc32(const vps_tensor* x, const vps_tensor* offse
                     y->c == cout, "deform_conv_tc32: shapes");
   VPS_CHECK_ARG((int64_t)x->n * x->h * x->w * x->cs < (1ll << 31), "deform_conv_tc32: tensor too large for 32-bit offsets");
   VPS_CHECK_ARG(((uintptr_t)w & 127) == 0, "deform_conv_tc32: weights not aligned");
-  auto encode = get_encode32();
-  if (!encode) { vps::set_error("cuTensorMapEncodeTiled unavailable"); return VPS_E_CUDA; }
+  auto encode = vps::tensor_map_encoder();
+  if (!encode) return VPS_E_CUDA;
   VPS_CHECK_ARG(y->dtype == VPS_F32, "deform_conv_tc32: y must be fp32");
   Dcn32Plan g;
   const int st = dcn32_plan(x->n, x->h, x->w, x->c, cout, g);
@@ -1072,19 +899,15 @@ extern "C" int vps_deform_conv_tc32(const vps_tensor* x, const vps_tensor* offse
   p.kh = p.kw = 3; p.sh = p.sw = 1; p.halo = 0; p.halo_w = 0;
   p.cin_chunks = x->c / T32_KC;
   e.rows = g.rows; e.dcn = 1; e.dcn_split_n = g.split_n;
-  e.plane_bytes = g.rows * 64; e.stage_bytes = 0; e.nk_last = 2;
+  e.plane_bytes = g.rows * 64; e.stage_bytes = 0; p.nk_last = 2;
   e.b_plane_bytes = block_n * 64;
   p.a_box_bytes = 0; p.a_stage_bytes = T32_PLANES * e.plane_bytes;
   p.a_stages = g.a_stages; p.b_stages = g.b_stages;
   p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
   p.total_tiles = p.tiles_per_prob;
-  p.y = y->ptr; p.y_h = y->h; p.y_w = y->w; p.y_cs = y->cs; p.y_dtype = y->dtype;
-  const int esz = y->dtype == VPS_BF16 ? 2 : 4;
-  p.y_vec = (((uintptr_t)y->ptr & 15) == 0) && ((y->cs * esz) % 16 == 0);
-  if (p.y_vec && (((uintptr_t)y->ptr & 31) == 0) && ((y->cs * esz) % 32 == 0)) p.y_vec = 2;
+  set_output(p, *y);
   p.oy_mul = p.ox_mul = 1;
-  p.res = nullptr; p.bias = nullptr; p.cout = cout; p.act = VPS_ACT_NONE; p.slope = 0.f; p.out_scale = 1.f;
-  p.stats = nullptr;
+  p.cout = cout; p.act = VPS_ACT_NONE; p.out_scale = 1.f;
   if (p.total_tiles == 0) return VPS_OK;
   Dcn32Params d;
   d.x = (const float*)x->ptr; d.off = (const float*)offset->ptr; d.x_cs = x->cs; d.off_cs = offset->cs; d.H = x->h; d.W = x->w;
@@ -1099,30 +922,14 @@ extern "C" int vps_deform_conv_tc32(const vps_tensor* x, const vps_tensor* offse
                         CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { vps::set_error("deform_conv_tc32: encode B failed (%d)", (int)r); return VPS_E_CUDA; }
   }
-  const int smem = g.smem;
-  static bool smem_set = false;
-  if (!smem_set) {
-    if (cudaFuncSetAttribute(dcn_igemm_tc32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
-      vps::set_error("deform_conv_tc32: cannot raise dynamic smem: %s", cudaGetErrorString(cudaGetLastError()));
-      return VPS_E_CUDA;
-    }
-    // a hint only: the driver picks the smallest carve-out that holds the launch's dynamic shared memory (<= DCN32_SMEM_MAX)
+  // a hint only: the driver picks the smallest carve-out that holds the launch's dynamic shared memory (<= DCN32_SMEM_MAX)
+  static bool carveout_set = false;
+  if (!carveout_set) {
     cudaFuncSetAttribute(dcn_igemm_tc32_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 58);
     (void)cudaGetLastError();
-    smem_set = true;
+    carveout_set = true;
   }
-  const int grid = p.total_tiles < g_num_sms32 ? p.total_tiles : g_num_sms32;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(DCN32_THREADS); cfg.dynamicSmemBytes = (size_t)smem;
-  cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  const cudaError_t le = cudaLaunchKernelEx(&cfg, dcn_igemm_tc32_kernel, tmB, p, e, d);
-  if (le != cudaSuccess) { vps::set_error("deform_conv_tc32: launch failed: %s", cudaGetErrorString(le)); return VPS_E_CUDA; }
-  VPS_CUDA_LAST("dcn_igemm_tc32_kernel");
-  return VPS_OK;
+  return launch_persistent<dcn_igemm_tc32_kernel>(p.total_tiles, DCN32_THREADS, g.smem, stream, "deform_conv_tc32", tmB, p, e, d);
 }
 
 extern "C" int vps_deform_conv_tc32_plan(const vps_tensor* x, int cout, int* plan) {

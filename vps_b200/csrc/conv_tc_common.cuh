@@ -1,8 +1,9 @@
-// Shared device code of the wgmma implicit-GEMM kernels (conv_tc.cu: bf16 operands; conv_tc32.cu: fp32 operands split on
-// the fly into fp16 main + correction planes): launch parameters, PTX wrappers (mbarrier / TMA), shared-memory matrix
-// descriptors, and the epilogue (register accumulators -> bias / activation / residual -> NHWC store).
+// Shared code of the wgmma kernels (conv_tc.cu: bf16 operands; conv_tc32.cu: fp32 operands split on the fly into fp16 main +
+// correction planes; corr_tc.cu): launch parameters, PTX wrappers (mbarrier / TMA), shared-memory matrix descriptors, the fp16
+// operand split, the DCN sampling set-up, the epilogue (register accumulators -> bias / activation / residual -> NHWC store),
+// and the host side common to the convolution launchers.
 #pragma once
-#include <cudaTypedefs.h>
+#include <cuda_fp16.h>
 
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -21,7 +22,7 @@ struct ConvTcParams {
   int n_img, oh, ow;
   int th, tw, tiles_y, tiles_x;
   int n_tiles_n, block_n;
-  int kh, kw, sh, sw, ph, pw;
+  int kh, kw, sh, sw;
   int cin_chunks;
   int a_stages, b_stages;     // operand rings (A: activation boxes, B: weight boxes)
   int halo;                   // 1: one (th+kh-1) x (tw+kw-1) activation box per channel chunk feeds all kh*kw taps
@@ -32,10 +33,9 @@ struct ConvTcParams {
   int gsub;                   // flat (non-halo) mode: K steps per ring slot (one barrier round covers gsub steps)
   int nk_last;                // K16 slabs of the last channel chunk that hold real channels (the rest is zero padding)
   int total_tiles;
-  long long* stats;           // optional [grid][8] clock counters (VPS_CONV_STATS=1), else NULL
   void* y;
   int y_h, y_w, y_cs, y_dtype, y_vec;
-  int oy_mul, oy_off, ox_mul, ox_off;
+  int oy_mul, ox_mul;
   const void* res;
   int res_cs, res_dtype, res_after_act, res_vec;
   const float* bias;
@@ -89,6 +89,14 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, uint
       "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_5d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, int c3,
+                                            int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
+      "%4, %5, %6, %7}], [%2];" ::"r"(dst),
+      "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+}
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
@@ -102,6 +110,12 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, uint
       "%4}], [%2];" ::"r"(dst),
       "l"(tmap), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
+}
+// shared -> global tensor store of one box (clipped at the tensor bounds), in the issuing thread's bulk async-group
+__device__ __forceinline__ void tma_store_4d(const void* tmap, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(tmap), "r"(src),
+               "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
 }
 // true in exactly one lane of the (converged) warp -- the same lane every time for a full mask
 __device__ __forceinline__ bool elect_one() {
@@ -126,6 +140,81 @@ __host__ __device__ __forceinline__ uint64_t desc_hi(uint32_t row_bytes, uint32_
   return d;
 }
 __device__ __forceinline__ uint64_t desc_at(uint64_t hi, uint32_t smem_addr) { return hi | (uint64_t)((smem_addr & 0x3FFFF) >> 4); }
+
+// ---------------------------------------------------------------- fp16 operand split of the fp32-parity precision
+// v = hi + 2^-11 lo:  hi = fp16(v),  lo = fp16(2^11 (v - hi))  (round to nearest, saturating; see conv_tc32.cu)
+constexpr float T32_LO_SCALE = 2048.f, T32_LO_INV = 1.f / 2048.f;
+
+// |v| > 65504 (or NaN): outside the fp16 range, so the split saturates hi
+__device__ __forceinline__ bool f16_over(float v) { return !(fabsf(v) <= 65504.f); }
+
+// split of one value (round to nearest, saturating).  The range check is left to the caller (f16_over): with a flag passed
+// by reference the compiler no longer folds the checks of consecutive values into one predicate chain.
+__device__ __forceinline__ void split_f16(float v, unsigned short& hi, unsigned short& lo) {
+  asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(hi) : "f"(v));
+  const float r = (v - __half2float(__ushort_as_half(hi))) * T32_LO_SCALE;      // exact in fp32; never exceeds |v|
+  asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(lo) : "f"(r));
+}
+
+// split of two values at once: hi = packed fp16x2 of (v0, v1), lo = packed fp16x2 of 2^11 * (v - fp16(v)).  Same values as two
+// split_f16() calls with 10 instead of 14 instructions; `over` collects f16_over of both values (the converter and the deformable sampler are bound by exactly this
+// arithmetic).
+__device__ __forceinline__ void split_pair_f16(float v0, float v1, uint32_t& hi, uint32_t& lo, bool& over) {
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(v1), "f"(v0));       // first source -> upper half
+  over = over || !(fabsf(v0) <= 65504.f) || !(fabsf(v1) <= 65504.f);
+  const float2 h = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+  const float r0 = (v0 - h.x) * T32_LO_SCALE, r1 = (v1 - h.y) * T32_LO_SCALE;          // exact in fp32
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(r1), "f"(r0));
+}
+
+// ---------------------------------------------------------------- weight packing
+// element i of a packed [cout_pad][kh][kw][cin_pad] weight buffer: the source weight times scale[co] (if given), 0 in the
+// padding; src OIHW, or IOHW when transposed
+__device__ __forceinline__ float packed_weight(const float* __restrict__ src, const float* __restrict__ scale, int64_t i, int cout,
+                                               int cin, int kh, int kw, int cin_pad, int transposed) {
+  const int ci = (int)(i % cin_pad);
+  int64_t t = i / cin_pad;
+  const int s = (int)(t % kw); t /= kw;
+  const int r = (int)(t % kh); t /= kh;
+  const int co = (int)t;
+  float v = 0.f;
+  if (co < cout && ci < cin) {
+    const int64_t si = transposed ? ((((int64_t)ci * cout + co) * kh + r) * kw + s) : ((((int64_t)co * cin + ci) * kh + r) * kw + s);
+    v = src[si];
+    if (scale) v *= scale[co];
+  }
+  return v;
+}
+
+// ---------------------------------------------------------------- deformable convolution (DCNv1, 3x3, pad 1)
+// Sampling set-up of tap k of output pixel (yo, xo) of image img -- the 4 bilinear corner weights and the 4 element offsets of
+// the corners in x (0 / 0 outside the image) -- as one 32-byte shared-memory entry at `sa`.  D: the kernel's DCN parameters
+// (off, off_cs, x_cs, H, W).
+template <class D>
+__device__ __forceinline__ void dcn_setup_entry(const D& d, uint32_t sa, int img, int yo, int xo, int k) {
+  const int H = d.H, W = d.W;
+  float wts[4] = {0.f, 0.f, 0.f, 0.f};
+  int offs[4] = {0, 0, 0, 0};
+  if (yo < H && xo < W) {
+    const float* op = d.off + ((int64_t)(img * H + yo) * W + xo) * d.off_cs;
+    const float oh = __ldg(op + 2 * k), ow = __ldg(op + 2 * k + 1);
+    const float h = (float)(yo - 1 + k / 3) + oh;
+    const float w = (float)(xo - 1 + k % 3) + ow;
+    if (h > -1.f && w > -1.f && h < (float)H && w < (float)W) {
+      const int hl = (int)floorf(h), wl = (int)floorf(w);
+      const int hh_ = hl + 1, wh_ = wl + 1;
+      const float lh = h - (float)hl, lw = w - (float)wl;
+      const float hh = 1.f - lh, hw = 1.f - lw;
+      const int base = img * H;
+      if (hl >= 0 && wl >= 0) { wts[0] = hh * hw; offs[0] = ((base + hl) * W + wl) * d.x_cs; }
+      if (hl >= 0 && wh_ <= W - 1) { wts[1] = hh * lw; offs[1] = ((base + hl) * W + wh_) * d.x_cs; }
+      if (hh_ <= H - 1 && wl >= 0) { wts[2] = lh * hw; offs[2] = ((base + hh_) * W + wl) * d.x_cs; }
+      if (hh_ <= H - 1 && wh_ <= W - 1) { wts[3] = lh * lw; offs[3] = ((base + hh_) * W + wh_) * d.x_cs; }
+    }
+  }
+  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(sa), "f"(wts[0]), "f"(wts[1]), "f"(wts[2]), "f"(wts[3]) : "memory");
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sa + 16u), "r"(offs[0]), "r"(offs[1]), "r"(offs[2]), "r"(offs[3]) : "memory");
+}
 
 // ---------------------------------------------------------------- tile walk shared by the roles
 struct TileCoord {
@@ -246,6 +335,77 @@ __device__ __forceinline__ void epi_frag(const ConvTcParams& p, const float (&d)
       }
     }
   }
+}
+
+// ---------------------------------------------------------------- host
+// Width of the output patch of `pixels` pixels (tw x pixels / tw) with the smallest padded area over oh x ow.  The first
+// minimum in candidate order wins; a candidate whose TMA box extents tw * sw or th * sh exceed 256 is skipped.
+inline int patch_tw(int oh, int ow, int pixels, int sh, int sw) {
+  int best_tw = 16;
+  int64_t best_area = -1;
+  for (const int tw : {16, 8, 32, 64, 128, 256}) {
+    const int th = pixels / tw;
+    if (th == 0 || tw * sw > 256 || th * sh > 256) continue;
+    const int64_t area = (int64_t)vps::cdiv(ow, tw) * tw * vps::cdiv(oh, th) * th;
+    if (best_area < 0 || area < best_area) { best_area = area; best_tw = tw; }
+  }
+  return best_tw;
+}
+
+// the output tensor of the epilogue; pair stores are 128-bit (y_vec 1) or 256-bit (y_vec 2) aligned where the layout allows
+inline void set_output(ConvTcParams& p, const vps_tensor& y) {
+  p.y = y.ptr; p.y_h = y.h; p.y_w = y.w; p.y_cs = y.cs; p.y_dtype = y.dtype;
+  const int esz = y.dtype == VPS_BF16 ? 2 : 4;
+  p.y_vec = (((uintptr_t)y.ptr & 15) == 0) && ((y.cs * esz) % 16 == 0);
+  if (p.y_vec && (((uintptr_t)y.ptr & 31) == 0) && ((y.cs * esz) % 32 == 0)) p.y_vec = 2;
+}
+
+// Padding, output mapping and epilogue of the nprob problems of one convolution launch; `who` prefixes the error messages.
+inline int set_problems(ConvTcParams& p, const vps_conv_args* args, int nprob, const char* who) {
+  const vps_conv_args* a = &args[0];
+  set_output(p, a->y);
+  p.oy_mul = a->oy_mul; p.ox_mul = a->ox_mul;
+  for (int i = 0; i < MAX_PROB; ++i) {
+    const vps_conv_args* q = &args[i < nprob ? i : 0];
+    p.ph_[i] = q->ph; p.pw_[i] = q->pw; p.oy_off_[i] = q->oy_off; p.ox_off_[i] = q->ox_off;
+    VPS_CHECK_ARG((a->oh - 1) * a->oy_mul + q->oy_off < a->y.h && (a->ow - 1) * a->ox_mul + q->ox_off < a->y.w,
+                  "%s: output mapping out of range", who);
+  }
+  p.res = a->res.ptr; p.res_cs = a->res.cs; p.res_dtype = a->res.dtype; p.res_after_act = a->res_after_act;
+  p.res_vec = a->res.ptr && (((uintptr_t)a->res.ptr & 15) == 0) && (a->res.cs % 8 == 0);
+  if (p.res_vec && (((uintptr_t)a->res.ptr & 31) == 0) && (a->res.cs % 16 == 0)) p.res_vec = 2;       // 256-bit loads
+  VPS_CHECK_ARG(!a->bias || ((uintptr_t)a->bias & 15) == 0, "%s: bias must be 16-byte aligned", who);
+  p.bias = a->bias; p.cout = a->cout; p.act = a->act; p.slope = a->slope; p.out_scale = a->out_scale;
+  if (a->res.ptr) VPS_CHECK_ARG(a->res.h == a->y.h && a->res.w == a->y.w, "%s: residual geometry", who);
+  return VPS_OK;
+}
+
+// Persistent launch of the tile kernel K: grid = min(tiles, SMs), with programmatic stream serialization, so that the kernel's
+// prologue (barrier init, tensor-map prefetch) overlaps the previous kernel's tail until its griddepcontrol.wait.  Only for
+// kernels that execute griddepcontrol.wait before they touch global memory.  The dynamic shared-memory limit is raised once
+// per kernel.  `who` prefixes the error messages.
+template <auto K, typename... A>
+int launch_persistent(int tiles, int threads, int smem, void* stream, const char* who, const A&... args) {
+  static bool smem_raised = false;
+  if (!smem_raised) {
+    if (cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
+      vps::set_error("%s: cannot raise dynamic smem: %s", who, cudaGetErrorString(cudaGetLastError()));
+      return VPS_E_CUDA;
+    }
+    smem_raised = true;
+  }
+  const int sms = vps::num_sms();
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)(tiles < sms ? tiles : sms)); cfg.blockDim = dim3((unsigned)threads);
+  cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = (cudaStream_t)stream;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr.val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = &attr; cfg.numAttrs = 1;
+  const cudaError_t le = cudaLaunchKernelEx(&cfg, K, args...);
+  if (le != cudaSuccess) { vps::set_error("%s: launch failed: %s", who, cudaGetErrorString(le)); return VPS_E_CUDA; }
+  VPS_CUDA_LAST(who);
+  return VPS_OK;
 }
 
 }  // namespace

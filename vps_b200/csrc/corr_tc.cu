@@ -12,11 +12,7 @@
 //
 //   warp 0         : TMA producer (f1 tile resident & double-buffered per tile; f2 blocks streamed through a 6-stage ring)
 //   warpgroups 1, 2: wgmma + band extraction
-#include <cudaTypedefs.h>
-#include <cuda_fp16.h>
-
-#include "common.cuh"
-#include "wgmma.cuh"
+#include "conv_tc_common.cuh"
 
 namespace {
 
@@ -37,43 +33,6 @@ struct CorrParams {
   int accumulate;     // 1: add to the fp32 value already in `out` before the activation
   int f16;            // 1: fp16 operands (the split planes of fp32 features), 0: bf16
 };
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// retry loop inside the PTX block (no divergent C++ loop or call between wgmma batches); traps after 2^26 failed polls
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n.reg .pred p;\n.reg .u32 n;\nmov.u32 n, 0;\n"
-      "VPS_WAIT:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra.uni VPS_DONE;\n"
-      "add.u32 n, n, 1;\n"
-      "setp.lt.u32 p, n, %2;\n"
-      "@p bra.uni VPS_WAIT;\n"
-      "trap;\n"
-      "VPS_DONE:\n}\n" ::"r"(bar), "r"(parity), "n"(1u << 26)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ uint64_t make_desc(uint32_t addr) {   // K-major, 128-byte rows, SWIZZLE_128B, 8-row groups 1 KiB apart
-  uint64_t d = (uint64_t)((addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 62;
-  return d;
-}
 
 // R = max_displacement / stride2, S2 = stride2.  TW = 32 - 2R so the neighbourhood is exactly 32 columns wide.
 template <int R, int S2, bool F16>
@@ -104,8 +63,9 @@ __device__ __forceinline__ void corr_consumer(const CorrParams& p, uint32_t a_ri
     for (int b = 0; b < NBLK; ++b) {
       for (int kc = 0; kc < p.kch; ++kc) {
         mbar_wait(afull(stage), phase);
-        const uint64_t adesc = make_desc(a_ring + stage * A_BYTES + (uint32_t)wg * 64u * 128u);
-        const uint64_t bdesc = make_desc(b_buf + bsel * MAX_KCH * B_BYTES + kc * B_BYTES);
+        // K-major, 128-byte rows (SWIZZLE_128B), 8-row groups 1 KiB apart
+        const uint64_t adesc = desc_at(desc_hi(128, 1024), a_ring + stage * A_BYTES + (uint32_t)wg * 64u * 128u);
+        const uint64_t bdesc = desc_at(desc_hi(128, 1024), b_buf + bsel * MAX_KCH * B_BYTES + kc * B_BYTES);
         wg::fence();
 #pragma unroll
         for (int k = 0; k < KC / 16; ++k)
@@ -214,31 +174,10 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmF1, const __grid_constant__
   }
 }
 
-PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-  if (!fn) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = (PFN_cuTensorMapEncodeTiled_v12000)ptr;
-  }
-  return fn;
-}
-
 template <int R, int S2>
 int launch(const vps_tensor* f1, const vps_tensor* f2, const vps_tensor* out, int act, float slope, cudaStream_t st,
            float scale = 0.f, int accumulate = 0, int f16 = 0) {
   constexpr int TW = 32 - 2 * R, TH = NPIX / TW;
-  auto encode = get_encode();
-  if (!encode) { vps::set_error("cuTensorMapEncodeTiled unavailable"); return VPS_E_CUDA; }
-  static int num_sms = 0;
-  if (!num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-  }
   CorrParams p;
   p.H = f1->h; p.W = f1->w; p.C = f1->c; p.kch = f1->c / KC; p.n_img = f1->n;
   p.tiles_y = vps::cdiv(vps::cdiv(f1->h, S2), TH);
@@ -246,19 +185,14 @@ int launch(const vps_tensor* f1, const vps_tensor* f2, const vps_tensor* out, in
   p.total_tiles = p.tiles_y * p.tiles_x * S2 * S2 * f1->n;
   p.out = out->ptr; p.out_cs = out->cs; p.out_dtype = out->dtype; p.act = act; p.slope = slope;
   p.scale = scale != 0.f ? scale : 1.0f / (float)f1->c; p.accumulate = accumulate; p.f16 = f16;
+  // f1: the tile's output pixels; f2: blocks of 4 rows x 32 columns of its neighbourhood (same-parity pixels)
+  const CUtensorMapDataType type = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   CUtensorMap tm1, tm2;
-  for (int which = 0; which < 2; ++which) {
-    const vps_tensor* t = which == 0 ? f1 : f2;
-    cuuint64_t dims[4] = {(cuuint64_t)t->c, (cuuint64_t)t->w, (cuuint64_t)t->h, (cuuint64_t)t->n};
-    cuuint64_t strides[3] = {(cuuint64_t)t->cs * 2, (cuuint64_t)t->w * t->cs * 2, (cuuint64_t)t->h * t->w * t->cs * 2};
-    cuuint32_t box1[4] = {KC, (cuuint32_t)(TW * S2), (cuuint32_t)(TH * S2), 1};
-    cuuint32_t box2[4] = {KC, (cuuint32_t)(32 * S2), (cuuint32_t)(4 * S2), 1};
-    cuuint32_t estr[4] = {1, S2, S2, 1};
-    CUresult r = encode(which == 0 ? &tm1 : &tm2, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, t->ptr, dims, strides,
-                        which == 0 ? box1 : box2, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                        CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { vps::set_error("correlation_tc: tensor map encode failed (%d)", (int)r); return VPS_E_CUDA; }
-  }
+  if (!vps::encode_nhwc(&tm1, *f1, type, KC, TW * S2, TH * S2, S2, S2, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                        "correlation_tc: encode f1") ||
+      !vps::encode_nhwc(&tm2, *f2, type, KC, 32 * S2, 4 * S2, S2, S2, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                        "correlation_tc: encode f2"))
+    return VPS_E_CUDA;
   const int smem = A_STAGES * A_BYTES + 2 * MAX_KCH * B_BYTES + 1024 + 8 * (2 * A_STAGES + 12);
   auto kern = corr_tc_kernel<R, S2>;
   static bool attr_set = false;
@@ -269,14 +203,16 @@ int launch(const vps_tensor* f1, const vps_tensor* f2, const vps_tensor* out, in
     }
     attr_set = true;
   }
-  const int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
+  // a plain launch: the kernel has no griddepcontrol.wait, so it must not start before the previous kernel has completed
+  const int sms = vps::num_sms();
+  const int grid = p.total_tiles < sms ? p.total_tiles : sms;
   kern<<<grid, 384, smem, st>>>(tm1, tm2, p);
   VPS_CUDA_LAST("corr_tc_kernel");
   return VPS_OK;
 }
 
 // fp32 features -> two fp16 planes (dense NHWC, cs = c):  hi = fp16(v),  lo = fp16(2^11 * (v - hi))  -- the operand split of the
-// fp32-parity convolutions (conv_tc32.cu): v = hi + 2^-11 * lo to ~2^-22 relative
+// fp32-parity convolutions (split_f16): v = hi + 2^-11 * lo to ~2^-22 relative
 __global__ void split_f16_planes_kernel(const float* __restrict__ x, int64_t npix, int c, int cs, __half* __restrict__ hi,
                                         __half* __restrict__ lo, unsigned int* overflow) {
   const int64_t total = npix * (c / 4);
@@ -290,10 +226,8 @@ __global__ void split_f16_planes_kernel(const float* __restrict__ x, int64_t npi
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       unsigned short hb, lb;
-      asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(hb) : "f"(vv[k]));
-      over = over || !(fabsf(vv[k]) <= 65504.f);
-      const float r = (vv[k] - __half2float(__ushort_as_half(hb))) * 2048.f;
-      asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(lb) : "f"(r));
+      split_f16(vv[k], hb, lb);
+      over = over || f16_over(vv[k]);
       h[k] = __ushort_as_half(hb); l[k] = __ushort_as_half(lb);
     }
     *reinterpret_cast<uint2*>(hi + pix * c + c4) = *reinterpret_cast<const uint2*>(h);
@@ -343,7 +277,7 @@ extern "C" int vps_correlation_tc32(const vps_tensor* f1, const vps_tensor* f2, 
   VPS_CUDA_LAST("split_f16_planes");
   split_f16_planes_kernel<<<blocks, 256, 0, st>>>((const float*)f2->ptr, npix, f1->c, f2->cs, base + 2 * plane, base + 3 * plane, flag);
   VPS_CUDA_LAST("split_f16_planes");
-  const float s1 = 1.0f / (float)f1->c, s2 = s1 * (1.0f / 2048.0f);
+  const float s1 = 1.0f / (float)f1->c, s2 = s1 * T32_LO_INV;
   int rc;
 #define CORR_PASS(A, B, SC, ACC, ACT)                                                                        \
   rc = (R == 10) ? launch<10, 2>(&t[A], &t[B], out, ACT, slope, st, SC, ACC, 1) : launch<4, 1>(&t[A], &t[B], out, ACT, slope, st, SC, ACC, 1); \
