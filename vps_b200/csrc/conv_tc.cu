@@ -20,19 +20,33 @@
 namespace {
 
 constexpr int NUM_THREADS = 384;     // warpgroup 0: warp 0 = TMA producer (warps 1-3 idle); warpgroups 1, 2: MMA + epilogue
+constexpr int TC_BAR_BYTES = 8 * (4 * MAX_STAGES + 8);
 
-
-// ---------------------------------------------------------------- TMA producer (warp 0)
-// The loop runs warp-uniformly and picks the issuing lane with elect.sync: code under `if (lane == 0)` is divergent to the
-// compiler, which then wraps every TMA instruction in a uniformity loop.  In halo mode one barrier round covers a whole
-// filter row (kw taps) when the row's weights fit one ring slot.
+// Shared memory of the bf16 kernels from the 1024-byte aligned `base`: A ring, B ring, the DCN's sampling set-up table, the
+// barriers.  smem = the launch's dynamic size, with 1 KB of slack for aligning the base.
 struct Ring {
-  uint32_t a_base, a_stage_bytes, b_base, b_stage_bytes, bar_base;
+  uint32_t a_base, a_stage_bytes, b_base, b_stage_bytes, setup_base, bar_base, smem;
   __device__ __forceinline__ uint32_t afull(int s) const { return bar_base + 8u * s; }
   __device__ __forceinline__ uint32_t aempty(int s) const { return bar_base + 8u * (MAX_STAGES + s); }
   __device__ __forceinline__ uint32_t bfull(int s) const { return bar_base + 8u * (2 * MAX_STAGES + s); }
   __device__ __forceinline__ uint32_t bempty(int s) const { return bar_base + 8u * (3 * MAX_STAGES + s); }
 };
+// a B slot holds the weights of one tap, of a filter row (halo mode, rowg) or of gsub K steps (flat mode)
+__host__ __device__ __forceinline__ Ring tc_ring(uint32_t base, const ConvTcParams& p, bool dcn) {
+  Ring rg;
+  rg.a_base = base; rg.a_stage_bytes = (uint32_t)p.a_stage_bytes;
+  rg.b_base = rg.a_base + (uint32_t)p.a_stages * rg.a_stage_bytes;
+  rg.b_stage_bytes = (uint32_t)p.block_n * ((uint32_t)p.bk * 2u) * (p.halo ? (p.rowg ? (uint32_t)p.kw : 1u) : (uint32_t)p.gsub);
+  rg.setup_base = rg.b_base + (uint32_t)p.b_stages * rg.b_stage_bytes;
+  rg.bar_base = rg.setup_base + (dcn ? (uint32_t)dcn_setup_bytes(BLOCK_M) : 0u);
+  rg.smem = rg.bar_base + TC_BAR_BYTES + 1024u - base;
+  return rg;
+}
+
+// ---------------------------------------------------------------- TMA producer (warp 0)
+// The loop runs warp-uniformly and picks the issuing lane with elect.sync: code under `if (lane == 0)` is divergent to the
+// compiler, which then wraps every TMA instruction in a uniformity loop.  In halo mode one barrier round covers a whole
+// filter row (kw taps) when the row's weights fit one ring slot.
 
 // ---- halo mode: one activation box per channel chunk (A ring), weights per tap or per filter row (B ring)
 template <bool ROWG>
@@ -41,27 +55,20 @@ __device__ __forceinline__ void producer_halo(const ConvTcParams& p, const Ring&
                                               const CUtensorMap* tmB3) {
   const int bk = p.bk, kw = p.kw, cin_chunks = p.cin_chunks, a_stages = p.a_stages, b_stages = p.b_stages;
   const int ngrp = ROWG ? p.kh : p.kh * p.kw;
-  const int tiles_per_img = p.tiles_y * p.tiles_x;
   const uint32_t a_box_bytes = (uint32_t)p.a_box_bytes;
   int as = 0, bs = 0;
   uint32_t aphase = 0, bphase = 0;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-    const int prob = tile / p.tiles_per_prob;
-    const int t_in = tile - prob * p.tiles_per_prob;
-    const int n_idx = t_in % p.n_tiles_n;
-    const int m_idx = t_in / p.n_tiles_n;
-    const int img = m_idx / tiles_per_img;
-    const int rem = m_idx - img * tiles_per_img;
-    const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
-    const int x_base = tx * p.tw - p.pw_[prob];
-    const int y_base = ty * p.th - p.ph_[prob];
-    const int n0 = n_idx * p.block_n;
-    const CUtensorMap* tmB = prob == 0 ? tmB0 : (prob == 1 ? tmB1 : (prob == 2 ? tmB2 : tmB3));
+    const TileCoord t = tile_coord(p, tile);
+    const int x_base = t.tx * p.tw - p.pw_[t.prob];
+    const int y_base = t.ty * p.th - p.ph_[t.prob];
+    const int n0 = t.n_idx * p.block_n;
+    const CUtensorMap* tmB = t.prob == 0 ? tmB0 : (t.prob == 1 ? tmB1 : (t.prob == 2 ? tmB2 : tmB3));
     for (int cc = 0; cc < cin_chunks; ++cc) {
       mbar_wait(rg.aempty(as), aphase ^ 1);
       if (elect_one()) {
         mbar_expect_tx(rg.afull(as), a_box_bytes);
-        tma_load_4d(rg.a_base + as * rg.a_stage_bytes, tmA, rg.afull(as), cc * bk, x_base, y_base, img);
+        tma_load_4d(rg.a_base + as * rg.a_stage_bytes, tmA, rg.afull(as), cc * bk, x_base, y_base, t.img);
       }
       if (++as == a_stages) { as = 0; aphase ^= 1; }
       for (int g = 0; g < ngrp; ++g) {
@@ -83,23 +90,16 @@ __device__ __forceinline__ void producer_flat(const ConvTcParams& p, const Ring&
                                               const CUtensorMap* tmB3) {
   const int bk = p.bk, kw = p.kw, kh = p.kh, stages = p.a_stages, G = p.gsub;
   const int T = p.cin_chunks * kh * kw;
-  const int tiles_per_img = p.tiles_y * p.tiles_x;
   const uint32_t a_box_bytes = (uint32_t)p.a_box_bytes;
   const uint32_t b_tile_bytes = (uint32_t)p.block_n * (uint32_t)bk * 2u;
   int st = 0;
   uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-    const int prob = tile / p.tiles_per_prob;
-    const int t_in = tile - prob * p.tiles_per_prob;
-    const int n_idx = t_in % p.n_tiles_n;
-    const int m_idx = t_in / p.n_tiles_n;
-    const int img = m_idx / tiles_per_img;
-    const int rem = m_idx - img * tiles_per_img;
-    const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
-    const int x_base = tx * p.tw * p.sw - p.pw_[prob];
-    const int y_base = ty * p.th * p.sh - p.ph_[prob];
-    const int n0 = n_idx * p.block_n;
-    const CUtensorMap* tmB = prob == 0 ? tmB0 : (prob == 1 ? tmB1 : (prob == 2 ? tmB2 : tmB3));
+    const TileCoord t = tile_coord(p, tile);
+    const int x_base = t.tx * p.tw * p.sw - p.pw_[t.prob];
+    const int y_base = t.ty * p.th * p.sh - p.ph_[t.prob];
+    const int n0 = t.n_idx * p.block_n;
+    const CUtensorMap* tmB = t.prob == 0 ? tmB0 : (t.prob == 1 ? tmB1 : (t.prob == 2 ? tmB2 : tmB3));
     int cc = 0, r = 0, sx = 0;
     for (int q0 = 0; q0 < T; q0 += G) {
       const int cnt = min(G, T - q0);
@@ -109,7 +109,7 @@ __device__ __forceinline__ void producer_flat(const ConvTcParams& p, const Ring&
       __syncwarp();
       for (int j = 0; j < cnt; ++j) {
         if (elect_one()) {
-          tma_load_4d(a_slot + j * a_box_bytes, tmA, rg.afull(st), cc * bk, x_base + sx, y_base + r, img);
+          tma_load_4d(a_slot + j * a_box_bytes, tmA, rg.afull(st), cc * bk, x_base + sx, y_base + r, t.img);
           tma_load_3d(b_slot + j * b_tile_bytes, tmB, rg.afull(st), cc * bk, n0, r * kw + sx);
         }
         if (++sx == kw) { sx = 0; if (++r == kh) { r = 0; ++cc; } }
@@ -243,22 +243,15 @@ conv_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
                      const __grid_constant__ CUtensorMap tmB3, const ConvTcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte aligned operand ring (SWIZZLE_128B requirement)
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t row_bytes = (uint32_t)p.bk * 2u;
-  const uint32_t a_stage_bytes = (uint32_t)p.a_stage_bytes;
-  const uint32_t b_stage_bytes = (uint32_t)p.block_n * row_bytes * (p.halo ? (p.rowg ? (uint32_t)p.kw : 1u) : (uint32_t)p.gsub);
-  const uint32_t b_base = smem_base + (uint32_t)p.a_stages * a_stage_bytes;
-  const uint32_t bar_base = b_base + (uint32_t)p.b_stages * b_stage_bytes;
+  // 1024-byte aligned operand ring (SWIZZLE_128B requirement)
+  const Ring rg = tc_ring((smem_u32(smem_raw) + 1023u) & ~1023u, p, false);
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);     // warp-uniform role index (wgmma issue is not treated as divergent)
   const int lane = threadIdx.x & 31;
-  Ring rg;
-  rg.a_base = smem_base; rg.a_stage_bytes = a_stage_bytes; rg.b_base = b_base; rg.b_stage_bytes = b_stage_bytes;
-  rg.bar_base = bar_base;
 
   // barrier slots (8 B each): afull, aempty, bfull, bempty [MAX_STAGES each]; full = one TMA arrival, empty = one arrival
   // per consumer warpgroup
   if (warp == 0) {
-    mbar_init(bar_base + 8u * lane, (lane >> 3) & 1 ? 2 : 1);
+    mbar_init(rg.bar_base + 8u * lane, (lane >> 3) & 1 ? 2 : 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (threadIdx.x == 32) {
@@ -294,16 +287,9 @@ conv_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
 constexpr int DCN_GATHER_WARPS = 7;
 constexpr int DCN_THREADS = 512;
 constexpr int DCN_MAX_N = 128;
-constexpr int DCN_SETUP_BYTES = 9 * BLOCK_M * 32;
 
-struct DcnParams {
-  const __nv_bfloat16* x;
-  const float* off;
-  int x_cs, off_cs, H, W;
-};
-
-__device__ __forceinline__ void dcn_gather_loop(const ConvTcParams& p, const DcnParams& d, const Ring& rg, uint32_t setup_base,
-                                                int gtid) {
+__device__ __forceinline__ void dcn_gather_loop(const ConvTcParams& p, const DcnParams<__nv_bfloat16>& d, const Ring& rg,
+                                                uint32_t setup_base, int gtid) {
   const int stages = p.a_stages, cin_chunks = p.cin_chunks;
   int st = 0;
   uint32_t phase = 0;
@@ -369,15 +355,9 @@ __device__ __forceinline__ void dcn_gather_loop(const ConvTcParams& p, const Dcn
 }
 
 __global__ void __launch_bounds__(DCN_THREADS, 1)
-dcn_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmB, const ConvTcParams p, const DcnParams d) {
+dcn_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmB, const ConvTcParams p, const DcnParams<__nv_bfloat16> d) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  Ring rg;
-  rg.a_base = smem_base; rg.a_stage_bytes = (uint32_t)p.a_stage_bytes;
-  rg.b_base = smem_base + (uint32_t)p.a_stages * rg.a_stage_bytes;
-  rg.b_stage_bytes = (uint32_t)p.block_n * 128u;
-  const uint32_t setup_base = rg.b_base + (uint32_t)p.a_stages * rg.b_stage_bytes;
-  rg.bar_base = setup_base + DCN_SETUP_BYTES;
+  const Ring rg = tc_ring((smem_u32(smem_raw) + 1023u) & ~1023u, p, true);
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);     // warp-uniform role index (wgmma issue is not treated as divergent)
   if (threadIdx.x == 0) {
     for (int s = 0; s < MAX_STAGES; ++s) {
@@ -414,7 +394,7 @@ dcn_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmB, const ConvTcParams 
         }
       }
     } else {
-      dcn_gather_loop(p, d, rg, setup_base, warp < 4 ? (int)threadIdx.x - 32 : (int)threadIdx.x - 384 + 96);
+      dcn_gather_loop(p, d, rg, rg.setup_base, warp < 4 ? (int)threadIdx.x - 32 : (int)threadIdx.x - 384 + 96);
     }
   }
 }
@@ -428,6 +408,23 @@ __global__ void pack_weights_tc_kernel(const float* __restrict__ src, const floa
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
        i += (int64_t)gridDim.x * blockDim.x)
     dst[i] = __float2bfloat16_rn(packed_weight(src, scale, i, cout, cin, kh, kw, cin_pad, transposed));
+}
+
+// Packed weights [cout_pad][taps][cin_pad] viewed as {cin_pad, cout_pad, taps}: a box is {bk, block_n, box_taps}, i.e.
+// consecutive K-major [block_n][bk] tiles, one per tap.  `who` prefixes the error message.
+bool encode_weights_tc(CUtensorMap* m, const void* w, int cout, int taps, int cin_pad, int bk, int block_n, int box_taps,
+                       const char* who) {
+  const auto encode = vps::tensor_map_encoder();
+  if (!encode) return false;
+  cuuint64_t dims[3] = {(cuuint64_t)cin_pad, (cuuint64_t)((cout + 15) / 16 * 16), (cuuint64_t)taps};
+  cuuint64_t strides[2] = {(cuuint64_t)taps * cin_pad * 2, (cuuint64_t)cin_pad * 2};
+  cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)block_n, (cuuint32_t)box_taps};
+  cuuint32_t estr[3] = {1, 1, 1};
+  const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)w, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { vps::set_error("%s: encode B failed (%d)", who, (int)r); return false; }
+  return true;
 }
 
 }  // namespace
@@ -468,8 +465,6 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
                       args[i].cin_gran == a->cin_gran,
                   "conv2d_tc_multi: problems must share geometry");
   }
-  auto encode = vps::tensor_map_encoder();
-  if (!encode) return VPS_E_CUDA;
   const int sms = vps::num_sms();
   if (sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
 
@@ -478,24 +473,21 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
   p.bk = bk;
   const int cin_pad = cin_pad_for(a->cin, bk);
   const int cout_pad = (a->cout + 15) / 16 * 16;
-  p.n_img = a->x.n; p.oh = a->oh; p.ow = a->ow;
   // halo mode (stride 1, more than one tap): the 8 rows of an MMA row group are 8 consecutive pixels of one halo row,
   // so the tile is 16 x 8 pixels and every tap reads the same (16+kh-1) x (8+kw-1) box at a shifted start address.
   const bool halo = a->sh == 1 && a->sw == 1 && a->kh * a->kw > 1 && a->kh <= 8 && a->kw <= 8;
   p.halo = halo ? 1 : 0;
-  p.tw = halo ? 8 : patch_tw(a->oh, a->ow, BLOCK_M, a->sh, a->sw);
-  p.th = BLOCK_M / p.tw;
-  p.halo_w = p.tw + a->kw - 1;
-  const int halo_h = p.th + a->kh - 1;
+  const int tw = halo ? 8 : patch_tw(a->oh, a->ow, BLOCK_M, a->sh, a->sw), th = BLOCK_M / tw;
+  p.halo_w = tw + a->kw - 1;
+  const int halo_h = th + a->kh - 1;
   p.a_box_bytes = halo ? halo_h * p.halo_w * bk * 2 : BLOCK_M * bk * 2;
   p.a_stage_bytes = (p.a_box_bytes + 1023) / 1024 * 1024;
-  p.tiles_x = vps::cdiv(a->ow, p.tw); p.tiles_y = vps::cdiv(a->oh, p.th);
   // N tile: pick the divisor of cout_pad (multiple of 16, <= 256) that minimises a simple time model
   //   waves(bn) * k_steps * max(fixed per-step latency, MMA time 2*bn clk, stage bytes / per-SM L2 bandwidth)
   // -- large tiles when there is enough parallelism, smaller N tiles to fill the persistent grid otherwise.
   int block_n = 16;
   {
-    const int64_t m_tiles = (int64_t)a->x.n * p.tiles_y * p.tiles_x * nprob;
+    const int64_t m_tiles = (int64_t)a->x.n * vps::cdiv(a->oh, th) * vps::cdiv(a->ow, tw) * nprob;
     double best = -1.0;
     for (int bn = 16; bn <= 256 && bn <= cout_pad; bn *= 2) {     // the N extents the consumer is instantiated for
       if (cout_pad % bn) continue;
@@ -513,9 +505,7 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
       if (best < 0 || t < best * 0.999) { best = t; block_n = bn; }
     }
   }
-  p.block_n = block_n; p.n_tiles_n = cout_pad / block_n;
-  p.kh = a->kh; p.kw = a->kw; p.sh = a->sh; p.sw = a->sw;
-  p.cin_chunks = cin_pad / bk;
+  set_tiles(p, a, nprob, tw, th, block_n, bk);
   // halo mode: one B ring slot = the kw taps of a filter row when that fits (<= 48 KB) -- one barrier round per row
   p.rowg = (halo && a->kw > 1 && a->kw * block_n * bk * 2 <= 48 * 1024) ? 1 : 0;
   p.nk_last = bk == 64 ? (a->cin - (p.cin_chunks - 1) * 64 + 15) / 16 : 1;
@@ -531,7 +521,7 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
     p.gsub = g;
     p.a_stage_bytes = g * p.a_box_bytes;
   }
-  const int b_stage_bytes = block_n * bk * 2 * (halo ? (p.rowg ? a->kw : 1) : p.gsub);
+  const int b_stage_bytes = (int)tc_ring(0, p, false).b_stage_bytes;
   if (halo) {
     p.a_stages = p.cin_chunks >= 3 ? 3 : 2;
     int bst = (200 * 1024 - p.a_stages * p.a_stage_bytes) / b_stage_bytes;
@@ -542,35 +532,21 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
     if (stages > MAX_STAGES) stages = MAX_STAGES;
     p.a_stages = p.b_stages = stages;
   }
-  p.nprob = nprob;
-  p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
-  p.total_tiles = p.tiles_per_prob * nprob;
   const int st = set_problems(p, args, nprob, "conv2d_tc");
   if (st != VPS_OK) return st;
   if (p.total_tiles == 0) return VPS_OK;
 
   CUtensorMap tmA, tmB[MAX_PROB];
-  const CUtensorMapSwizzle swz = bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_32B;
-  if (!vps::encode_nhwc(&tmA, a->x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, bk, halo ? p.halo_w : p.tw * a->sw,
-                        halo ? halo_h : p.th * a->sh, a->sw, a->sh, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "conv2d_tc: encode A"))
+  if (!vps::encode_nhwc(&tmA, a->x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, bk, halo ? p.halo_w : tw * a->sw, halo ? halo_h : th * a->sh,
+                        a->sw, a->sh, bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_32B,
+                        CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "conv2d_tc: encode A"))
     return VPS_E_CUDA;
-  for (int i = 0; i < MAX_PROB; ++i) {
-    const vps_conv_args* q = &args[i < nprob ? i : 0];
-    // packed weights [cout_pad][tap][cin_pad] viewed as {cin_pad, cout_pad, taps}: a box is {bk, block_n, taps-per-slot},
-    // i.e. consecutive K-major [block_n][bk] tiles, one per tap
-    const cuuint64_t K = (cuuint64_t)a->kh * a->kw * cin_pad;
-    cuuint64_t dims[3] = {(cuuint64_t)cin_pad, (cuuint64_t)cout_pad, (cuuint64_t)(a->kh * a->kw)};
-    cuuint64_t strides[2] = {K * 2, (cuuint64_t)cin_pad * 2};
-    cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)block_n, (cuuint32_t)(p.rowg ? a->kw : 1)};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = encode(&tmB[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)q->w, dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { vps::set_error("conv2d_tc: encode B failed (%d)", (int)r); return VPS_E_CUDA; }
-  }
-  const int smem = p.a_stages * p.a_stage_bytes + p.b_stages * b_stage_bytes + 1024 + 8 * (4 * MAX_STAGES + 8);
-  return launch_persistent<conv_igemm_tc_kernel>(p.total_tiles, NUM_THREADS, smem, stream, "conv2d_tc", tmA, tmB[0], tmB[1],
-                                                 tmB[2], tmB[3], p);
+  for (int i = 0; i < MAX_PROB; ++i)
+    if (!encode_weights_tc(&tmB[i], args[i < nprob ? i : 0].w, a->cout, a->kh * a->kw, cin_pad, bk, block_n, p.rowg ? a->kw : 1,
+                           "conv2d_tc"))
+      return VPS_E_CUDA;
+  return launch_persistent<conv_igemm_tc_kernel>(p.total_tiles, NUM_THREADS, (int)tc_ring(0, p, false).smem, stream, "conv2d_tc",
+                                                 tmA, tmB[0], tmB[1], tmB[2], tmB[3], p);
 }
 
 extern "C" int vps_conv2d_tc(const vps_conv_args* a, void* stream) { return vps_conv2d_tc_multi(a, 1, stream); }
@@ -588,46 +564,26 @@ extern "C" int vps_deform_conv_tc(const vps_tensor* x, const vps_tensor* offset,
   VPS_CHECK_ARG((int64_t)x->n * x->h * x->w * x->cs < (1ll << 31), "deform_conv_tc: tensor too large for 32-bit offsets");
   const int cout_pad = (cout + 15) / 16 * 16;
   VPS_CHECK_ARG(cout_pad <= 256 && ((uintptr_t)w & 15) == 0, "deform_conv_tc: cout %d > 256", cout);
-  auto encode = vps::tensor_map_encoder();
-  if (!encode) return VPS_E_CUDA;
   if (vps::num_sms() <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
+  vps_conv_args a = dcn_args(*x, cout);
+  a.y = *y;
   ConvTcParams p = {};
-  p.bk = 64; p.nprob = 1;
-  p.n_img = x->n; p.oh = x->h; p.ow = x->w;
-  p.tw = patch_tw(x->h, x->w, BLOCK_M, 1, 1); p.th = BLOCK_M / p.tw;
-  p.tiles_x = vps::cdiv(x->w, p.tw); p.tiles_y = vps::cdiv(x->h, p.th);
+  p.bk = 64;
   // weight rows past cout_pad are TMA zero fill
-  p.block_n = cout_pad <= 64 ? 64 : DCN_MAX_N;
-  p.n_tiles_n = vps::cdiv(cout_pad, p.block_n);
-  p.kh = p.kw = 3; p.sh = p.sw = 1;
-  p.cin_chunks = x->c / 64;
-  p.gsub = 1; p.nk_last = 4; p.halo = 0; p.rowg = 0;
+  const int tw = patch_tw(x->h, x->w, BLOCK_M, 1, 1);
+  set_tiles(p, &a, 1, tw, BLOCK_M / tw, cout_pad <= 64 ? 64 : DCN_MAX_N, 64);
+  p.gsub = 1; p.nk_last = 4;
   p.a_box_bytes = BLOCK_M * 128; p.a_stage_bytes = p.a_box_bytes;
-  const int stage_bytes = p.a_stage_bytes + p.block_n * 128;
-  int stages = (200 * 1024 - DCN_SETUP_BYTES) / stage_bytes;
+  int stages = (200 * 1024 - dcn_setup_bytes(BLOCK_M)) / (p.a_stage_bytes + (int)tc_ring(0, p, true).b_stage_bytes);
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   VPS_CHECK_ARG(stages >= 2, "deform_conv_tc: ring does not fit");
   p.a_stages = p.b_stages = stages;
-  p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
-  p.total_tiles = p.tiles_per_prob;
-  set_output(p, *y);
-  p.oy_mul = p.ox_mul = 1;
-  p.cout = cout; p.act = VPS_ACT_NONE; p.out_scale = 1.f;
+  const int st = set_problems(p, &a, 1, "deform_conv_tc");
+  if (st != VPS_OK) return st;
   if (p.total_tiles == 0) return VPS_OK;
-  DcnParams d;
-  d.x = (const __nv_bfloat16*)x->ptr; d.off = (const float*)offset->ptr; d.x_cs = x->cs; d.off_cs = offset->cs;
-  d.H = x->h; d.W = x->w;
+  const DcnParams<__nv_bfloat16> d = {(const __nv_bfloat16*)x->ptr, (const float*)offset->ptr, x->cs, offset->cs, x->h, x->w};
   CUtensorMap tmB;
-  {
-    const cuuint64_t K = (cuuint64_t)9 * x->c;
-    cuuint64_t dims[3] = {(cuuint64_t)x->c, (cuuint64_t)cout_pad, 9};
-    cuuint64_t strides[2] = {K * 2, (cuuint64_t)x->c * 2};
-    cuuint32_t box[3] = {64, (cuuint32_t)p.block_n, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = encode(&tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)w, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { vps::set_error("deform_conv_tc: encode B failed (%d)", (int)r); return VPS_E_CUDA; }
-  }
-  const int smem = stages * stage_bytes + DCN_SETUP_BYTES + 1024 + 8 * (4 * MAX_STAGES + 8);
-  return launch_persistent<dcn_igemm_tc_kernel>(p.total_tiles, DCN_THREADS, smem, stream, "deform_conv_tc", tmB, p, d);
+  if (!encode_weights_tc(&tmB, w, cout, 9, x->c, 64, p.block_n, 1, "deform_conv_tc")) return VPS_E_CUDA;
+  return launch_persistent<dcn_igemm_tc_kernel>(p.total_tiles, DCN_THREADS, (int)tc_ring(0, p, true).smem, stream, "deform_conv_tc",
+                                                tmB, p, d);
 }

@@ -61,12 +61,6 @@ struct Tc32Extra {
   int dcn_split_n;           // DCN split-N layout: the consumer warpgroups share the tile's pixels, each takes block_n / 2 channels
 };
 
-struct Dcn32Params {
-  const float* x;
-  const float* off;
-  int x_cs, off_cs, H, W;
-};
-constexpr int dcn32_setup_bytes(int rows) { return 9 * rows * 32; }    // per (tap, pixel): 4 bilinear weights + 4 element offsets
 // the fused DCN kernel is bound by its sampling warps (CUDA-core issue + L1 latency), so it runs 4 warpgroups: warp 0 = weight
 // TMA, warps 1-3 and 12-15 = 7 sampling warps, warpgroups 1 and 2 = consumers.  setmaxnreg moves registers from warpgroups 0
 // and 3 to the consumers, whose 176 hold the step accumulator and the promoted sum at N = 128 per warpgroup.  Each sample is
@@ -89,7 +83,9 @@ struct Ring32 {
   uint32_t a_base, a_bytes;      // operand-plane ring (T32_PLANES planes per slot)
   uint32_t b_base, b_bytes;      // weight ring (T32_PLANES planes per slot)
   uint32_t e_base, bias_base;    // TMA epilogue: the consumers' output boxes, their block_n bias values
+  uint32_t setup_base;           // DCN: the tile's sampling set-up table
   uint32_t bar_base;
+  uint32_t smem;                 // the launch's dynamic shared memory: all of the above + 1 KB of slack for aligning the base
   __device__ __forceinline__ uint32_t sfull(int s) const { return bar_base + 8u * s; }
   __device__ __forceinline__ uint32_t sempty(int s) const { return bar_base + 8u * (MAX_STAGES + s); }
   __device__ __forceinline__ uint32_t pfull(int s) const { return bar_base + 8u * (2 * MAX_STAGES + s); }
@@ -107,7 +103,23 @@ constexpr int t32_box_c(int n) { return n >= 32 ? 32 : 16; }
 // At N = 128 the sum alone takes 64 of the 168 registers of a 384-thread CTA, and the TMA epilogue's unrolled pass over it
 // spills around the slow-path call of the sigmoid's IEEE division; those tiles keep the fragment epilogue.
 constexpr int T32_EPI_MAX_N = 64;
-constexpr int t32_epi_bytes(int nwg, int bn) { return 64 * nwg * bn * 4 + nwg * bn * 4; }    // output boxes + bias
+
+// Shared memory of the tc32 kernels from the 1024-byte aligned `base`, in this order: the convolution's staging ring,
+// operand-plane ring, weight ring, with the TMA epilogue the output boxes and bias of the nwg consumer warpgroups, the DCN's
+// set-up table, then the barriers.  The ring slots are multiples of 1 KB, so every region after them is 1024-byte aligned.
+__host__ __device__ __forceinline__ Ring32 ring32(uint32_t base, const ConvTcParams& p, const Tc32Extra& e, int nwg, bool epi_tma,
+                                                  bool dcn) {
+  Ring32 rg;
+  rg.s_base = base; rg.s_bytes = dcn ? 0u : (uint32_t)e.stage_bytes;
+  rg.a_base = rg.s_base + T32_STAGE_SLOTS * rg.s_bytes; rg.a_bytes = (uint32_t)T32_PLANES * (uint32_t)e.plane_bytes;
+  rg.b_base = rg.a_base + (uint32_t)p.a_stages * rg.a_bytes; rg.b_bytes = (uint32_t)T32_PLANES * (uint32_t)e.b_plane_bytes;
+  rg.e_base = rg.b_base + (uint32_t)p.b_stages * rg.b_bytes;
+  rg.bias_base = rg.e_base + (epi_tma ? 64u * nwg * (uint32_t)p.block_n * 4u : 0u);
+  rg.setup_base = rg.bias_base + (epi_tma ? (uint32_t)nwg * (uint32_t)p.block_n * 4u : 0u);
+  rg.bar_base = rg.setup_base + (dcn ? (uint32_t)dcn_setup_bytes(e.rows) : 0u);
+  rg.smem = rg.bar_base + T32_BAR_BYTES + 1024u - base;
+  return rg;
+}
 
 // ---------------------------------------------------------------- warp 0: TMA producer
 __device__ __forceinline__ void producer32(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, const CUtensorMap* tmA,
@@ -198,7 +210,7 @@ __device__ __forceinline__ void converter32(const ConvTcParams& p, const Tc32Ext
 // fp16 planes straight into the operand ring -- the 9x column matrix (1.2 GB per P2 layer in fp32) never exists.  K steps run
 // chunk-major / tap-minor: the nine taps of a 32-channel chunk re-read the same few KB of input from L1.  A tile has e.rows
 // (128 or 64) pixels, i.e. e.rows / 8 sampling units per K step.
-__device__ __forceinline__ void dcn_gather32(const ConvTcParams& p, const Tc32Extra& e, const Dcn32Params& d, const Ring32& rg,
+__device__ __forceinline__ void dcn_gather32(const ConvTcParams& p, const Tc32Extra& e, const DcnParams<float>& d, const Ring32& rg,
                                              uint32_t setup_base, uint32_t ctr_addr, int gtid) {
   constexpr int NT = 32 * DCN32_GATHER_WARPS;
   const int lane = gtid & 31;
@@ -469,14 +481,7 @@ conv_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                        const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmR, const ConvTcParams p,
                        const Tc32Extra e) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  Ring32 rg;
-  rg.s_base = smem_base; rg.s_bytes = (uint32_t)e.stage_bytes;
-  rg.a_base = rg.s_base + T32_STAGE_SLOTS * rg.s_bytes; rg.a_bytes = (uint32_t)T32_PLANES * (uint32_t)e.plane_bytes;
-  rg.b_base = rg.a_base + (uint32_t)p.a_stages * rg.a_bytes; rg.b_bytes = (uint32_t)T32_PLANES * (uint32_t)e.b_plane_bytes;
-  rg.e_base = rg.b_base + (uint32_t)p.b_stages * rg.b_bytes;          // 1024-aligned: the ring slots are multiples of 1 KB
-  rg.bias_base = rg.e_base + (TMA_EPI ? 64u * NWG * (uint32_t)p.block_n * 4u : 0u);
-  rg.bar_base = rg.bias_base + (TMA_EPI ? (uint32_t)NWG * (uint32_t)p.block_n * 4u : 0u);
+  const Ring32 rg = ring32((smem_u32(smem_raw) + 1023u) & ~1023u, p, e, NWG, TMA_EPI, false);
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);     // warp-uniform role index (wgmma issue is not treated as divergent)
   if (warp == 0) init_bars32(rg, 32 * T32_CONV_WARPS, 32 * T32_CONV_WARPS, NWG);
   if (threadIdx.x == 32) {
@@ -498,15 +503,9 @@ conv_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 
 // ---------------------------------------------------------------- fused DCNv1 kernel (same pipeline, sampling warps feed the ring)
 __global__ void __launch_bounds__(DCN32_THREADS, 1)
-dcn_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmB, const ConvTcParams p, const Tc32Extra e, const Dcn32Params d) {
+dcn_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmB, const ConvTcParams p, const Tc32Extra e, const DcnParams<float> d) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  Ring32 rg;
-  rg.s_base = smem_base; rg.s_bytes = 0;
-  rg.a_base = smem_base; rg.a_bytes = (uint32_t)T32_PLANES * (uint32_t)e.plane_bytes;
-  rg.b_base = rg.a_base + (uint32_t)p.a_stages * rg.a_bytes; rg.b_bytes = (uint32_t)T32_PLANES * (uint32_t)e.b_plane_bytes;
-  const uint32_t setup_base = rg.b_base + (uint32_t)p.b_stages * rg.b_bytes;
-  rg.bar_base = setup_base + dcn32_setup_bytes(e.rows);
+  const Ring32 rg = ring32((smem_u32(smem_raw) + 1023u) & ~1023u, p, e, 2, false, true);
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);     // warp-uniform role index (wgmma issue is not treated as divergent)
   if (warp == 0) init_bars32(rg, (uint32_t)e.rows / 8u, 1, 2);
   if (threadIdx.x == 32) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
@@ -528,7 +527,7 @@ dcn_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmB, const ConvTcParam
   } else {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(DCN32_LO_REGS));
     if (warp == 0) producer32(p, e, rg, &tmB, &tmB);
-    else dcn_gather32(p, e, d, rg, setup_base, rg.unit_ctr(), warp < 4 ? (int)threadIdx.x - 32 : (int)threadIdx.x - 384 + 96);
+    else dcn_gather32(p, e, d, rg, rg.setup_base, rg.unit_ctr(), warp < 4 ? (int)threadIdx.x - 32 : (int)threadIdx.x - 384 + 96);
   }
 }
 
@@ -555,17 +554,34 @@ inline int64_t plane_elems(int cout, int cin, int kh, int kw) {
   return cout_pad * kh * kw * cin_pad;
 }
 
-constexpr int T32_SMEM_BUDGET = 227 * 1024 - 1024 - T32_BAR_BYTES - 64;
+// Packed weights [plane][prob][cout_pad][tap][cin_pad] (vps_pack_weights_tc32): a box is {T32_KC channels, block_n rows} of
+// one tap and problem in both planes.  `who` prefixes the error message.
+bool encode_weights_tc32(CUtensorMap* m, const void* w, int nprob, int cout, int taps, int cin_pad, int block_n, const char* who) {
+  const auto encode = vps::tensor_map_encoder();
+  if (!encode) return false;
+  const int cout_pad = (cout + 15) / 16 * 16;
+  const int64_t n_plane = (int64_t)cout_pad * taps * cin_pad;
+  cuuint64_t dims[5] = {(cuuint64_t)cin_pad, (cuuint64_t)cout_pad, (cuuint64_t)taps, (cuuint64_t)nprob, T32_PLANES};
+  cuuint64_t strides[4] = {(cuuint64_t)taps * cin_pad * 2, (cuuint64_t)cin_pad * 2, (cuuint64_t)n_plane * 2,
+                           (cuuint64_t)n_plane * nprob * 2};
+  cuuint32_t box[5] = {(cuuint32_t)T32_KC, (cuuint32_t)block_n, 1, 1, T32_PLANES};
+  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 5, (void*)w, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { vps::set_error("%s: encode B failed (%d)", who, (int)r); return false; }
+  return true;
+}
 
-// Tiling of one tc32 launch.  Everything here follows from the shapes (and the SM count); vps_conv2d_tc32_multi launches
-// exactly this plan and vps_conv2d_tc32_plan reports it.
+constexpr int T32_SMEM_MAX = 227 * 1024 - 64;    // dynamic shared memory of a tc32 convolution
+
+// One tc32 launch: the kernel parameters and the choices only the host needs.  Everything here follows from the shapes (and
+// the SM count); the launchers launch exactly this plan and the plan queries report it.
 struct Tc32Plan {
-  int nwg;                   // consumer warpgroups: the tile holds 64 * nwg output pixels
-  int block_n;
-  int halo, tw, th, halo_w, halo_h;
-  int rows, stage_bytes, plane_bytes, a_stages, a_side;    // A item rows, staging / operand-plane slot bytes, ring depth
-  int b_stages;
+  ConvTcParams p;
+  Tc32Extra e;
+  int nwg;                   // convolution: consumer warpgroups, the tile holds 64 * nwg output pixels
   int epi_tma;               // 1: TMA epilogue (output boxes in shared memory), 0: stores from the accumulator fragments
+  int smem;                  // dynamic shared memory
 };
 
 // A tensor map can express the output (and the residual) of one problem written at unit output strides into fp32 tensors
@@ -580,21 +596,24 @@ bool tc32_epi_expressible(const vps_conv_args* a, int nprob) {
   return true;
 }
 
-Tc32Plan tc32_tile(const vps_conv_args* a, int nwg) {
+// The tile of nwg consumer warpgroups x block_n channels and its A items; tc32_plan sets the weight ring depth.
+Tc32Plan tc32_tile(const vps_conv_args* a, int nprob, int nwg, int block_n) {
   Tc32Plan g = {};
+  ConvTcParams& p = g.p;
   g.nwg = nwg;
   const int px = 64 * nwg;
-  g.halo = a->sh == 1 && a->sw == 1 && a->kh * a->kw > 1 && a->kh <= 8 && a->kw <= 8;
+  p.halo = a->sh == 1 && a->sw == 1 && a->kh * a->kw > 1 && a->kh <= 8 && a->kw <= 8;
   // 8-pixel halo rows: the consumer's descriptors step one halo row per 8-row group
-  g.tw = g.halo ? 8 : patch_tw(a->oh, a->ow, px, a->sh, a->sw);
-  g.th = px / g.tw;
-  g.halo_w = g.tw + a->kw - 1;
-  g.halo_h = g.th + a->kh - 1;
-  g.rows = g.halo ? g.halo_h * g.halo_w : px;
-  g.stage_bytes = (g.rows * 128 + 1023) / 1024 * 1024;
-  g.plane_bytes = (g.rows * 64 + 1023) / 1024 * 1024;
-  g.a_stages = g.halo ? 2 : 3;
-  g.a_side = T32_STAGE_SLOTS * g.stage_bytes + g.a_stages * T32_PLANES * g.plane_bytes;
+  const int tw = p.halo ? 8 : patch_tw(a->oh, a->ow, px, a->sh, a->sw);
+  set_tiles(p, a, nprob, tw, px / tw, block_n, T32_KC);
+  p.halo_w = tw + a->kw - 1;
+  p.nk_last = (a->cin - (p.cin_chunks - 1) * T32_KC + 15) / 16;
+  p.a_stages = p.halo ? 2 : 3;
+  g.e.rows = p.halo ? (p.th + a->kh - 1) * p.halo_w : px;
+  p.a_box_bytes = g.e.rows * 128;
+  g.e.stage_bytes = (g.e.rows * 128 + 1023) / 1024 * 1024;
+  g.e.plane_bytes = (g.e.rows * 64 + 1023) / 1024 * 1024;
+  g.e.b_plane_bytes = block_n * 64;
   return g;
 }
 
@@ -620,20 +639,19 @@ int tc32_plan(const vps_conv_args* a, int nprob, Tc32Plan& out) {
   const int steps = (a->cin + T32_KC - 1) / T32_KC * a->kh * a->kw;
   double best = -1.0;
   for (int nwg = 2; nwg <= 4; nwg += 2) {
-    Tc32Plan g = tc32_tile(a, nwg);
-    const int64_t m_tiles = (int64_t)a->x.n * vps::cdiv(a->oh, g.th) * vps::cdiv(a->ow, g.tw) * nprob;
-    const double conv = 2.0 * (g.halo ? (double)g.rows / (a->kh * a->kw) : (double)g.rows);
     for (int bn = 16; bn <= (nwg == 2 ? T32_MAX_N : T32_WIDE_MAX_N) && bn <= cout_pad; bn *= 2) {
       if (cout_pad % bn) continue;
-      if (g.a_side + 2 * bn * 64 * T32_PLANES > T32_SMEM_BUDGET) continue;
-      const int64_t tiles = m_tiles * (cout_pad / bn);
+      Tc32Plan g = tc32_tile(a, nprob, nwg, bn);
+      g.p.b_stages = 2;
+      if ((int)ring32(0, g.p, g.e, nwg, false, false).smem > T32_SMEM_MAX) continue;
+      const int64_t tiles = g.p.total_tiles;
       const double waves = (double)((tiles + sms - 1) / sms);
+      const double conv = 2.0 * (g.p.halo ? (double)g.e.rows / (a->kh * a->kw) : (double)g.e.rows);
       const double step = fmax(fmax(300.0, 1.5 * nwg * bn), fmax((double)(bn * 64 * T32_PLANES) / 56.0, conv));
       const double t = waves * ((double)steps * step + 40.0 * bn + 1500.0);
       if (best < 0 || t < best * 0.999) {
         best = t;
         out = g;
-        out.block_n = bn;
       }
     }
   }
@@ -646,32 +664,24 @@ int tc32_plan(const vps_conv_args* a, int nprob, Tc32Plan& out) {
   // stages, giving up the third operand-plane slot if need be (NWG 4 at block_n 64: 256-pixel A items).  Halo tiles keep the
   // fragment epilogue: they run tens of K steps per tile, and the boxes would take the weight stages their taps stream
   // through (NWG 4 at block_n 32 drops from 6 to 2 and ran 13-16% slower; per-layer H100 timings in DESIGN.md §5.0).
-  const int eb = t32_epi_bytes(out.nwg, out.block_n), b2 = 2 * T32_PLANES * out.block_n * 64;
-  out.epi_tma = 0;
-  if (!out.halo && out.block_n <= T32_EPI_MAX_N && tc32_epi_expressible(a, nprob)) {
-    if (out.a_side + b2 + eb > T32_SMEM_BUDGET && out.a_stages == 3 &&
-        out.a_side - T32_PLANES * out.plane_bytes + b2 + eb <= T32_SMEM_BUDGET) {
-      out.a_stages = 2;
-      out.a_side -= T32_PLANES * out.plane_bytes;
+  ConvTcParams& p = out.p;
+  p.b_stages = 2;
+  const auto epi_fits = [&] { return (int)ring32(0, p, out.e, out.nwg, true, false).smem <= T32_SMEM_MAX; };
+  if (!p.halo && p.block_n <= T32_EPI_MAX_N && tc32_epi_expressible(a, nprob)) {
+    if (!epi_fits() && p.a_stages == 3) {
+      p.a_stages = 2;
+      if (!epi_fits()) p.a_stages = 3;
     }
-    out.epi_tma = out.a_side + b2 + eb <= T32_SMEM_BUDGET;
+    out.epi_tma = epi_fits();
   }
-  const int bst = (T32_SMEM_BUDGET - out.a_side - (out.epi_tma ? eb : 0)) / (T32_PLANES * out.block_n * 64);
-  out.b_stages = bst > MAX_STAGES ? MAX_STAGES : bst;
+  p.b_stages = 0;
+  const Ring32 rg = ring32(0, p, out.e, out.nwg, out.epi_tma, false);
+  const int bst = (T32_SMEM_MAX - (int)rg.smem) / (int)rg.b_bytes;
+  p.b_stages = bst > MAX_STAGES ? MAX_STAGES : bst;
+  out.smem = (int)ring32(0, p, out.e, out.nwg, out.epi_tma, false).smem;
   return VPS_OK;
 }
 
-// Tiling of one fused DCN launch.  Everything follows from the shapes (and the SM count); vps_deform_conv_tc32 launches exactly
-// this plan and vps_deform_conv_tc32_plan reports it.
-struct Dcn32Plan {
-  int rows;                  // tile pixels: 128 (split-M) or 64 (split-N)
-  int split_n;
-  int bn;                    // channels per consumer warpgroup
-  int block_n;               // channels per tile: bn (split-M) or 2 bn (split-N)
-  int n_tiles;               // cout_pad / block_n
-  int tw, th;
-  int a_stages, b_stages, smem;
-};
 // Shared memory stays at most 132 KB so that L1 keeps room: the sampling warps read 4 x 128 B per (tap, pixel, 32-channel
 // chunk) through L1, and the nine taps of a chunk re-read the same ~60 KB footprint of the tile.
 constexpr int DCN32_SMEM_MAX = 132 * 1024;
@@ -685,38 +695,39 @@ constexpr double DCN32_UNIT_CLK = 220.0, DCN32_STEP_CLK = 300.0;
 // m64 x bn x k16 (6 bn clocks of the tensor pipe); the weight tile (2 planes x block_n x 64 B) at the L2 rate of 56 B/clk.
 // Every N tile samples the same input again, so a tile as wide as cout_pad samples each input once; narrower tiles win where
 // the grid would otherwise leave SMs idle.  Equal costs go to the plan that samples less.
-int dcn32_plan(int n, int h, int w, int cin, int cout, Dcn32Plan& out) {
+int dcn32_plan(const vps_conv_args* a, Tc32Plan& out) {
   const int sms = vps::num_sms();
   if (sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
-  const int cout_pad = (cout + 15) / 16 * 16;
-  const int steps = cin / T32_KC * 9;
+  const int cout_pad = (a->cout + 15) / 16 * 16;
+  const int steps = a->cin / T32_KC * 9;
   double best = -1.0, best_units = 0.0;
   for (int split_n = 0; split_n <= 1; ++split_n) {
-    const int rows = split_n ? 64 : 128;
-    const int best_tw = patch_tw(h, w, rows, 1, 1);
-    const int64_t m_tiles = (int64_t)n * vps::cdiv(h, rows / best_tw) * vps::cdiv(w, best_tw);
-    const int a_side = 2 * T32_PLANES * rows * 64 + dcn32_setup_bytes(rows);
+    const int rows = split_n ? 64 : 128;        // tile pixels: split-M or split-N
+    const int tw = patch_tw(a->oh, a->ow, rows, 1, 1);
     for (int bn = 16; bn <= DCN32_MAX_N; bn *= 2) {
       const int block_n = split_n ? 2 * bn : bn;
       if (block_n > cout_pad || cout_pad % block_n) continue;
-      const int b_slot = T32_PLANES * block_n * 64;
-      const int bst = (DCN32_SMEM_MAX - 1024 - T32_BAR_BYTES - a_side) / b_slot;
+      Tc32Plan g = {};
+      set_tiles(g.p, a, 1, tw, rows / tw, block_n, T32_KC);
+      g.p.nk_last = 2; g.p.a_stages = 2;
+      g.e.rows = rows; g.e.plane_bytes = rows * 64; g.e.b_plane_bytes = block_n * 64; g.e.dcn = 1; g.e.dcn_split_n = split_n;
+      const Ring32 rg = ring32(0, g.p, g.e, 2, false, true);
+      const int bst = (DCN32_SMEM_MAX - (int)rg.smem) / (int)rg.b_bytes;
       if (bst < 2) continue;
-      const int64_t tiles = m_tiles * (cout_pad / block_n);
+      const int64_t tiles = g.p.total_tiles;
       const double waves = (double)((tiles + sms - 1) / sms);
-      const double step = fmax(fmax(rows / 8 * DCN32_UNIT_CLK, fmax(DCN32_STEP_CLK, 6.0 * bn)), b_slot / 56.0);
+      const double step = fmax(fmax(rows / 8 * DCN32_UNIT_CLK, fmax(DCN32_STEP_CLK, 6.0 * bn)), rg.b_bytes / 56.0);
       const double t = waves * ((double)steps * step + 40.0 * bn + 1500.0), units = waves * rows;
       if (best < 0 || t < best * 0.999 || (t <= best * 1.001 && units < best_units)) {
         best = t; best_units = units;
-        out.rows = rows; out.split_n = split_n; out.bn = bn; out.block_n = block_n; out.n_tiles = cout_pad / block_n;
-        out.tw = best_tw; out.th = rows / best_tw;
-        out.a_stages = 2; out.b_stages = bst > 3 ? 3 : bst;
-        out.smem = a_side + out.b_stages * b_slot + 1024 + T32_BAR_BYTES;
+        g.p.b_stages = bst > 3 ? 3 : bst;
+        g.smem = (int)ring32(0, g.p, g.e, 2, false, true).smem;
+        out = g;
       }
     }
   }
   if (best < 0) {
-    vps::set_error("deform_conv_tc32: no tiling fits (cout %d)", cout);
+    vps::set_error("deform_conv_tc32: no tiling fits (cout %d)", a->cout);
     return VPS_E_ARG;
   }
   return VPS_OK;
@@ -776,67 +787,28 @@ extern "C" int vps_conv2d_tc32_multi(const vps_conv_args* args, int nprob, void*
                       args[i].bias == a->bias && args[i].act == a->act && args[i].oy_mul == a->oy_mul && args[i].ox_mul == a->ox_mul,
                   "conv2d_tc32_multi: problems must share geometry and the packed weight buffer");
   }
-  auto encode = vps::tensor_map_encoder();
-  if (!encode) return VPS_E_CUDA;
   Tc32Plan g;
   int st = tc32_plan(a, nprob, g);
   if (st != VPS_OK) return st;
-  VPS_CHECK_ARG(g.b_stages >= 2, "conv2d_tc32: ring does not fit (%d x %d px halo, bn %d)", g.halo_h, g.halo_w, g.block_n);
-  ConvTcParams p = {};
-  Tc32Extra e = {};
-  p.bk = T32_KC;
-  const int cin_pad = (a->cin + T32_KC - 1) / T32_KC * T32_KC;
-  const int cout_pad = (a->cout + 15) / 16 * 16;
-  p.n_img = a->x.n; p.oh = a->oh; p.ow = a->ow;
-  const bool halo = g.halo != 0;
-  p.halo = g.halo;
-  p.tw = g.tw; p.th = g.th;
-  p.halo_w = g.halo_w;
-  const int halo_h = g.halo_h;
-  e.rows = g.rows;
-  p.a_box_bytes = e.rows * 128;
-  e.stage_bytes = g.stage_bytes;
-  e.plane_bytes = g.plane_bytes;
-  p.a_stage_bytes = T32_PLANES * e.plane_bytes;
-  p.tiles_x = vps::cdiv(a->ow, p.tw); p.tiles_y = vps::cdiv(a->oh, p.th);
-  p.kh = a->kh; p.kw = a->kw; p.sh = a->sh; p.sw = a->sw;
-  p.cin_chunks = cin_pad / T32_KC;
-  const int rem = a->cin - (p.cin_chunks - 1) * T32_KC;
-  p.nk_last = (rem + 15) / 16;
-  const int ntaps = a->kh * a->kw;
-  p.a_stages = g.a_stages;
-  const int block_n = g.block_n;
-  p.block_n = block_n; p.n_tiles_n = cout_pad / block_n;
-  e.b_plane_bytes = block_n * 64;
-  p.b_stages = g.b_stages;
-  p.nprob = nprob;
-  p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
-  p.total_tiles = p.tiles_per_prob * nprob;
+  ConvTcParams& p = g.p;
+  const int halo_h = p.th + p.kh - 1;
+  VPS_CHECK_ARG(p.b_stages >= 2, "conv2d_tc32: ring does not fit (%d x %d px halo, bn %d)", halo_h, p.halo_w, p.block_n);
   st = set_problems(p, args, nprob, "conv2d_tc32");
   if (st != VPS_OK) return st;
   if (p.total_tiles == 0) return VPS_OK;
 
   CUtensorMap tmA, tmB;
-  if (!vps::encode_nhwc(&tmA, a->x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, T32_KC, halo ? p.halo_w : p.tw * a->sw,
-                        halo ? halo_h : p.th * a->sh, a->sw, a->sh, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+  if (!vps::encode_nhwc(&tmA, a->x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, T32_KC, p.halo ? p.halo_w : p.tw * a->sw,
+                        p.halo ? halo_h : p.th * a->sh, a->sw, a->sh, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                         "conv2d_tc32: encode A"))
     return VPS_E_CUDA;
-  const int64_t n_plane = (int64_t)cout_pad * ntaps * cin_pad;
-  {
-    cuuint64_t dims[5] = {(cuuint64_t)cin_pad, (cuuint64_t)cout_pad, (cuuint64_t)ntaps, (cuuint64_t)nprob, T32_PLANES};
-    cuuint64_t strides[4] = {(cuuint64_t)ntaps * cin_pad * 2, (cuuint64_t)cin_pad * 2, (cuuint64_t)n_plane * 2,
-                             (cuuint64_t)n_plane * nprob * 2};
-    cuuint32_t box[5] = {(cuuint32_t)T32_KC, (cuuint32_t)block_n, 1, 1, T32_PLANES};
-    cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    CUresult r = encode(&tmB, CU_TENSOR_MAP_DATA_TYPE_UINT16, 5, (void*)a->w, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { vps::set_error("conv2d_tc32: encode B failed (%d)", (int)r); return VPS_E_CUDA; }
-  }
+  if (!encode_weights_tc32(&tmB, a->w, nprob, a->cout, a->kh * a->kw, p.cin_chunks * T32_KC, p.block_n, "conv2d_tc32"))
+    return VPS_E_CUDA;
   // TMA epilogue: output and residual as [n][oh][ow][cout] from the first output pixel (a channel slice of a wider tensor
   // keeps its pixel stride); TMA clips the boxes at oh / ow / cout, so partial tiles and the neighbouring channels are safe
   CUtensorMap tmY = {}, tmR = {};
   if (g.epi_tma) {
-    const int bc = t32_box_c(block_n), box_w = p.tw < 64 ? p.tw : 64;
+    const int bc = t32_box_c(p.block_n), box_w = p.tw < 64 ? p.tw : 64;
     const int64_t px = (int64_t)a->oy_off * a->y.w + a->ox_off;
     for (int m = 0; m < (a->res.ptr ? 2 : 1); ++m) {
       const vps_tensor& t = m ? a->res : a->y;          // the residual has the output's geometry
@@ -848,11 +820,9 @@ extern "C" int vps_conv2d_tc32_multi(const vps_conv_args* args, int nprob, void*
         return VPS_E_CUDA;
     }
   }
-  const int smem = g.a_side + p.b_stages * T32_PLANES * e.b_plane_bytes + (g.epi_tma ? t32_epi_bytes(g.nwg, block_n) : 0) + 1024 +
-                   T32_BAR_BYTES;
 #define VPS_TC32_LAUNCH(NWG, EPI)                                                                                              \
-  launch_persistent<conv_igemm_tc32_kernel<NWG, EPI>>(p.total_tiles, t32_threads(NWG), smem, stream, "conv2d_tc32", tmA, tmB, tmY, \
-                                                      tmR, p, e)
+  launch_persistent<conv_igemm_tc32_kernel<NWG, EPI>>(p.total_tiles, t32_threads(NWG), g.smem, stream, "conv2d_tc32", tmA, tmB,  \
+                                                      tmY, tmR, p, g.e)
   if (g.nwg == 4) return g.epi_tma ? VPS_TC32_LAUNCH(4, true) : VPS_TC32_LAUNCH(4, false);
   return g.epi_tma ? VPS_TC32_LAUNCH(2, true) : VPS_TC32_LAUNCH(2, false);
 #undef VPS_TC32_LAUNCH
@@ -864,7 +834,7 @@ extern "C" int vps_conv2d_tc32_plan(const vps_conv_args* a, int nprob, int* plan
   Tc32Plan g;
   const int st = tc32_plan(a, nprob, g);
   if (st != VPS_OK) return st;
-  plan[0] = g.nwg; plan[1] = g.block_n; plan[2] = g.tw; plan[3] = g.th; plan[4] = g.halo; plan[5] = g.epi_tma;
+  plan[0] = g.nwg; plan[1] = g.p.block_n; plan[2] = g.p.tw; plan[3] = g.p.th; plan[4] = g.p.halo; plan[5] = g.epi_tma;
   return VPS_OK;
 }
 
@@ -881,47 +851,18 @@ extern "C" int vps_deform_conv_tc32(const vps_tensor* x, const vps_tensor* offse
                     y->c == cout, "deform_conv_tc32: shapes");
   VPS_CHECK_ARG((int64_t)x->n * x->h * x->w * x->cs < (1ll << 31), "deform_conv_tc32: tensor too large for 32-bit offsets");
   VPS_CHECK_ARG(((uintptr_t)w & 127) == 0, "deform_conv_tc32: weights not aligned");
-  auto encode = vps::tensor_map_encoder();
-  if (!encode) return VPS_E_CUDA;
   VPS_CHECK_ARG(y->dtype == VPS_F32, "deform_conv_tc32: y must be fp32");
-  Dcn32Plan g;
-  const int st = dcn32_plan(x->n, x->h, x->w, x->c, cout, g);
+  vps_conv_args a = dcn_args(*x, cout);
+  a.y = *y;
+  Tc32Plan g;
+  int st = dcn32_plan(&a, g);
   if (st != VPS_OK) return st;
-  const int cout_pad = (cout + 15) / 16 * 16;
-  ConvTcParams p = {};
-  Tc32Extra e = {};
-  p.bk = T32_KC; p.nprob = 1;
-  p.n_img = x->n; p.oh = x->h; p.ow = x->w;
-  p.tw = g.tw; p.th = g.th;
-  p.tiles_x = vps::cdiv(x->w, p.tw); p.tiles_y = vps::cdiv(x->h, p.th);
-  const int block_n = g.block_n;
-  p.block_n = block_n; p.n_tiles_n = g.n_tiles;
-  p.kh = p.kw = 3; p.sh = p.sw = 1; p.halo = 0; p.halo_w = 0;
-  p.cin_chunks = x->c / T32_KC;
-  e.rows = g.rows; e.dcn = 1; e.dcn_split_n = g.split_n;
-  e.plane_bytes = g.rows * 64; e.stage_bytes = 0; p.nk_last = 2;
-  e.b_plane_bytes = block_n * 64;
-  p.a_box_bytes = 0; p.a_stage_bytes = T32_PLANES * e.plane_bytes;
-  p.a_stages = g.a_stages; p.b_stages = g.b_stages;
-  p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
-  p.total_tiles = p.tiles_per_prob;
-  set_output(p, *y);
-  p.oy_mul = p.ox_mul = 1;
-  p.cout = cout; p.act = VPS_ACT_NONE; p.out_scale = 1.f;
-  if (p.total_tiles == 0) return VPS_OK;
-  Dcn32Params d;
-  d.x = (const float*)x->ptr; d.off = (const float*)offset->ptr; d.x_cs = x->cs; d.off_cs = offset->cs; d.H = x->h; d.W = x->w;
+  st = set_problems(g.p, &a, 1, "deform_conv_tc32");
+  if (st != VPS_OK) return st;
+  if (g.p.total_tiles == 0) return VPS_OK;
+  const DcnParams<float> d = {(const float*)x->ptr, (const float*)offset->ptr, x->cs, offset->cs, x->h, x->w};
   CUtensorMap tmB;
-  {
-    const int64_t n_plane = (int64_t)cout_pad * 9 * x->c;
-    cuuint64_t dims[5] = {(cuuint64_t)x->c, (cuuint64_t)cout_pad, 9, 1, T32_PLANES};
-    cuuint64_t strides[4] = {(cuuint64_t)9 * x->c * 2, (cuuint64_t)x->c * 2, (cuuint64_t)n_plane * 2, (cuuint64_t)n_plane * 2};
-    cuuint32_t box[5] = {(cuuint32_t)T32_KC, (cuuint32_t)block_n, 1, 1, T32_PLANES};
-    cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    CUresult r = encode(&tmB, CU_TENSOR_MAP_DATA_TYPE_UINT16, 5, (void*)w, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { vps::set_error("deform_conv_tc32: encode B failed (%d)", (int)r); return VPS_E_CUDA; }
-  }
+  if (!encode_weights_tc32(&tmB, w, 1, cout, 9, x->c, g.p.block_n, "deform_conv_tc32")) return VPS_E_CUDA;
   // a hint only: the driver picks the smallest carve-out that holds the launch's dynamic shared memory (<= DCN32_SMEM_MAX)
   static bool carveout_set = false;
   if (!carveout_set) {
@@ -929,14 +870,16 @@ extern "C" int vps_deform_conv_tc32(const vps_tensor* x, const vps_tensor* offse
     (void)cudaGetLastError();
     carveout_set = true;
   }
-  return launch_persistent<dcn_igemm_tc32_kernel>(p.total_tiles, DCN32_THREADS, g.smem, stream, "deform_conv_tc32", tmB, p, e, d);
+  return launch_persistent<dcn_igemm_tc32_kernel>(g.p.total_tiles, DCN32_THREADS, g.smem, stream, "deform_conv_tc32", tmB, g.p, g.e,
+                                                  d);
 }
 
 extern "C" int vps_deform_conv_tc32_plan(const vps_tensor* x, int cout, int* plan) {
   VPS_CHECK_ARG(x->c % T32_KC == 0 && x->c > 0 && cout > 0, "deform_conv_tc32_plan: cin %d, cout %d", x->c, cout);
-  Dcn32Plan g;
-  const int st = dcn32_plan(x->n, x->h, x->w, x->c, cout, g);
+  const vps_conv_args a = dcn_args(*x, cout);
+  Tc32Plan g;
+  const int st = dcn32_plan(&a, g);
   if (st != VPS_OK) return st;
-  plan[0] = g.rows; plan[1] = g.bn; plan[2] = g.split_n; plan[3] = g.n_tiles;
+  plan[0] = g.e.rows; plan[1] = g.e.dcn_split_n ? g.p.block_n / 2 : g.p.block_n; plan[2] = g.e.dcn_split_n; plan[3] = g.p.n_tiles_n;
   return VPS_OK;
 }

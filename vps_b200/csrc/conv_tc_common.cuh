@@ -187,11 +187,20 @@ __device__ __forceinline__ float packed_weight(const float* __restrict__ src, co
 }
 
 // ---------------------------------------------------------------- deformable convolution (DCNv1, 3x3, pad 1)
+// input x (bf16 or fp32 NHWC) and the fp32 NHWC offsets, (dy, dx) per tap
+template <class T>
+struct DcnParams {
+  const T* x;
+  const float* off;
+  int x_cs, off_cs, H, W;
+};
+// bytes of a tile's sampling set-up table: one 32-byte entry (4 bilinear weights + 4 element offsets) per (tap, pixel)
+__host__ __device__ constexpr int dcn_setup_bytes(int rows) { return 9 * rows * 32; }
+
 // Sampling set-up of tap k of output pixel (yo, xo) of image img -- the 4 bilinear corner weights and the 4 element offsets of
-// the corners in x (0 / 0 outside the image) -- as one 32-byte shared-memory entry at `sa`.  D: the kernel's DCN parameters
-// (off, off_cs, x_cs, H, W).
-template <class D>
-__device__ __forceinline__ void dcn_setup_entry(const D& d, uint32_t sa, int img, int yo, int xo, int k) {
+// the corners in x (0 / 0 outside the image) -- as one 32-byte shared-memory entry at `sa`.
+template <class T>
+__device__ __forceinline__ void dcn_setup_entry(const DcnParams<T>& d, uint32_t sa, int img, int yo, int xo, int k) {
   const int H = d.H, W = d.W;
   float wts[4] = {0.f, 0.f, 0.f, 0.f};
   int offs[4] = {0, 0, 0, 0};
@@ -350,6 +359,31 @@ inline int patch_tw(int oh, int ow, int pixels, int sh, int sw) {
     if (best_area < 0 || area < best_area) { best_area = area; best_tw = tw; }
   }
   return best_tw;
+}
+
+// Tile walk of a launch: th x tw output pixels x block_n channels per tile, K in chunks of kc channels, nprob problems.
+inline void set_tiles(ConvTcParams& p, const vps_conv_args* a, int nprob, int tw, int th, int block_n, int kc) {
+  p.n_img = a->x.n; p.oh = a->oh; p.ow = a->ow;
+  p.tw = tw; p.th = th;
+  p.tiles_x = vps::cdiv(a->ow, tw); p.tiles_y = vps::cdiv(a->oh, th);
+  p.block_n = block_n; p.n_tiles_n = vps::cdiv((a->cout + 15) / 16 * 16, block_n);
+  p.kh = a->kh; p.kw = a->kw; p.sh = a->sh; p.sw = a->sw;
+  p.cin_chunks = vps::cdiv(a->cin, kc);
+  p.nprob = nprob;
+  p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
+  p.total_tiles = p.tiles_per_prob * nprob;
+}
+
+// A DCN layer as the convolution whose tiles and epilogue it shares: 3x3, stride 1, pad 1, no bias, x's size.  The caller
+// sets the output y.
+inline vps_conv_args dcn_args(const vps_tensor& x, int cout) {
+  vps_conv_args a = {};
+  a.x = x;
+  a.kh = a.kw = 3; a.sh = a.sw = 1; a.ph = a.pw = 1;
+  a.oh = x.h; a.ow = x.w; a.oy_mul = a.ox_mul = 1;
+  a.cin = x.c; a.cout = cout;
+  a.act = VPS_ACT_NONE; a.out_scale = 1.f;
+  return a;
 }
 
 // the output tensor of the epilogue; pair stores are 128-bit (y_vec 1) or 256-bit (y_vec 2) aligned where the layout allows
