@@ -243,7 +243,6 @@ conv_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
                      const __grid_constant__ CUtensorMap tmB3, const ConvTcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte aligned operand ring (SWIZZLE_128B requirement)
-  // 1024-byte aligned operand ring (SWIZZLE_128B requirement)
   const Ring rg = tc_ring((smem_u32(smem_raw) + 1023u) & ~1023u, p, false);
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);     // warp-uniform role index (wgmma issue is not treated as divergent)
   const int lane = threadIdx.x & 31;

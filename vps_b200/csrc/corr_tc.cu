@@ -34,17 +34,38 @@ struct CorrParams {
   int f16;            // 1: fp16 operands (the split planes of fp32 features), 0: bf16
 };
 
-// R = max_displacement / stride2, S2 = stride2.  TW = 32 - 2R so the neighbourhood is exactly 32 columns wide.
+// Shared memory from the 1024-byte aligned `base`: f2 ring, two f1 tile buffers, barriers; smem = the launch's dynamic size
+struct CorrSmem {
+  uint32_t a_ring, b_buf, bars, smem;
+  __device__ __forceinline__ uint32_t afull(int s) const { return bars + 8u * s; }
+  __device__ __forceinline__ uint32_t aempty(int s) const { return bars + 8u * (A_STAGES + s); }
+  __device__ __forceinline__ uint32_t bfull(int s) const { return bars + 8u * (2 * A_STAGES + s); }
+  __device__ __forceinline__ uint32_t bempty(int s) const { return bars + 8u * (2 * A_STAGES + 2 + s); }
+};
+__host__ __device__ __forceinline__ CorrSmem corr_smem(uint32_t base) {
+  const uint32_t b_buf = base + A_STAGES * A_BYTES, bars = b_buf + 2 * MAX_KCH * B_BYTES;
+  return {base, b_buf, bars, bars + 8u * (2 * A_STAGES + 12) + 1024u - base};     // 2 * A_STAGES + 4 barriers used
+}
+
+// Tile `tile` (tiles_per_par per stride2-parity class): image, parity (py, px), first output pixel (y0, x0) less the parity
+struct CorrTile { int img, py, px, y0, x0; };
+template <int R, int S2>
+__device__ __forceinline__ CorrTile corr_tile(const CorrParams& p, int tiles_per_par, int tile) {
+  constexpr int TW = 32 - 2 * R, TH = NPIX / TW;
+  const int per_img = tiles_per_par * S2 * S2;
+  CorrTile c;
+  c.img = tile / per_img;
+  int t = tile - c.img * per_img;
+  const int par = t / tiles_per_par;
+  t -= par * tiles_per_par;
+  c.py = par / S2; c.px = par % S2;
+  c.y0 = (t / p.tiles_x) * TH * S2; c.x0 = (t % p.tiles_x) * TW * S2;
+  return c;
+}
+
 template <int R, int S2, bool F16>
-__device__ __forceinline__ void corr_consumer(const CorrParams& p, uint32_t a_ring, uint32_t b_buf, uint32_t bars, int wg) {
-  constexpr int D = 2 * R + 1;
-  constexpr int TW = 32 - 2 * R;
-  constexpr int TH = NPIX / TW;
-  constexpr int NBLK = (TH + 2 * R) / 4;
-  auto afull = [&](int s) { return bars + 8u * s; };
-  auto aempty = [&](int s) { return bars + 8u * (A_STAGES + s); };
-  auto bfull = [&](int s) { return bars + 8u * (2 * A_STAGES + s); };
-  auto bempty = [&](int s) { return bars + 8u * (2 * A_STAGES + 2 + s); };
+__device__ __forceinline__ void corr_consumer(const CorrParams& p, const CorrSmem& sm, int wg) {
+  constexpr int D = 2 * R + 1, TW = 32 - 2 * R, TH = NPIX / TW, NBLK = (TH + 2 * R) / 4;
   const bool leader = (threadIdx.x & 127) == 0;
   const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
   const int tiles_per_par = p.tiles_y * p.tiles_x;
@@ -52,27 +73,21 @@ __device__ __forceinline__ void corr_consumer(const CorrParams& p, uint32_t a_ri
   int bsel = 0; uint32_t bphase = 0;
   float d[NPIX / 2];
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-    const int per_img = tiles_per_par * S2 * S2;
-    const int img = tile / per_img;
-    int t = tile - img * per_img;
-    const int par = t / tiles_per_par;
-    t -= par * tiles_per_par;
-    const int py = par / S2, px = par % S2;
-    const int y0 = (t / p.tiles_x) * TH * S2, x0 = (t % p.tiles_x) * TW * S2;
-    mbar_wait(bfull(bsel), bphase);
+    const CorrTile t = corr_tile<R, S2>(p, tiles_per_par, tile);
+    mbar_wait(sm.bfull(bsel), bphase);
     for (int b = 0; b < NBLK; ++b) {
       for (int kc = 0; kc < p.kch; ++kc) {
-        mbar_wait(afull(stage), phase);
+        mbar_wait(sm.afull(stage), phase);
         // K-major, 128-byte rows (SWIZZLE_128B), 8-row groups 1 KiB apart
-        const uint64_t adesc = desc_at(desc_hi(128, 1024), a_ring + stage * A_BYTES + (uint32_t)wg * 64u * 128u);
-        const uint64_t bdesc = desc_at(desc_hi(128, 1024), b_buf + bsel * MAX_KCH * B_BYTES + kc * B_BYTES);
+        const uint64_t adesc = desc_at(desc_hi(128, 1024), sm.a_ring + stage * A_BYTES + (uint32_t)wg * 64u * 128u);
+        const uint64_t bdesc = desc_at(desc_hi(128, 1024), sm.b_buf + bsel * MAX_KCH * B_BYTES + kc * B_BYTES);
         wg::fence();
 #pragma unroll
         for (int k = 0; k < KC / 16; ++k)
           wg::Mma<NPIX, F16>::run(d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)((kc | k) != 0));
         wg::commit();
         wg::wait<0>();
-        if (leader) mbar_arrive(aempty(stage));
+        if (leader) mbar_arrive(sm.aempty(stage));
         if (++stage == A_STAGES) { stage = 0; phase ^= 1; }
       }
       wg::fence_regs(d);
@@ -92,10 +107,10 @@ __device__ __forceinline__ void corr_consumer(const CorrParams& p, uint32_t a_ri
             const int m = 8 * q + 2 * (ln & 3) + e;
             const int i = m / TW, j = m - (m / TW) * TW;
             const int tj = ip - i, ti = jp - j;
-            const int y = y0 + py + i * S2, x = x0 + px + j * S2;
+            const int y = t.y0 + t.py + i * S2, x = t.x0 + t.px + j * S2;
             if (tj >= 0 && tj < D && ti >= 0 && ti < D && y < p.H && x < p.W) {
               float v = d[4 * q + 2 * h + e] * p.scale;
-              const int64_t o = (((int64_t)img * p.H + y) * p.W + x) * p.out_cs + tj * D + ti;
+              const int64_t o = (((int64_t)t.img * p.H + y) * p.W + x) * p.out_cs + tj * D + ti;
               if (p.accumulate) v += ((const float*)p.out)[o];
               if (p.act == VPS_ACT_LRELU) v = v > 0.f ? v : v * p.slope;
               if (p.out_dtype == VPS_BF16) ((__nv_bfloat16*)p.out)[o] = __float2bfloat16_rn(v);
@@ -105,7 +120,7 @@ __device__ __forceinline__ void corr_consumer(const CorrParams& p, uint32_t a_ri
         }
       }
     }
-    if (leader) mbar_arrive(bempty(bsel));      // every MMA reading this f1 tile has completed
+    if (leader) mbar_arrive(sm.bempty(bsel));      // every MMA reading this f1 tile has completed
     bsel ^= 1; if (bsel == 0) bphase ^= 1;
   }
 }
@@ -114,25 +129,16 @@ __device__ __forceinline__ void corr_consumer(const CorrParams& p, uint32_t a_ri
 template <int R, int S2>
 __global__ void __launch_bounds__(384, 1)
 corr_tc_kernel(const __grid_constant__ CUtensorMap tmF1, const __grid_constant__ CUtensorMap tmF2, const CorrParams p) {
-  constexpr int TW = 32 - 2 * R;
-  constexpr int TH = NPIX / TW;
-  constexpr int NBLK = (TH + 2 * R) / 4;
+  constexpr int TW = 32 - 2 * R, TH = NPIX / TW, NBLK = (TH + 2 * R) / 4;
   static_assert(TW * TH == NPIX && (TH + 2 * R) % 4 == 0, "tile geometry");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t a_ring = base;                                   // A_STAGES x 16 KiB
-  const uint32_t b_buf = base + A_STAGES * A_BYTES;               // 2 x (kch x 12 KiB)
+  const CorrSmem sm = corr_smem((smem_u32(smem_raw) + 1023u) & ~1023u);
   const uint32_t b_tile_bytes = (uint32_t)p.kch * B_BYTES;
-  const uint32_t bars = b_buf + 2 * MAX_KCH * B_BYTES;
-  auto afull = [&](int s) { return bars + 8u * s; };
-  auto aempty = [&](int s) { return bars + 8u * (A_STAGES + s); };
-  auto bfull = [&](int s) { return bars + 8u * (2 * A_STAGES + s); };
-  auto bempty = [&](int s) { return bars + 8u * (2 * A_STAGES + 2 + s); };
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;     // warp-uniform role index
 
   if (threadIdx.x == 0) {      // full: one TMA arrival; empty: one arrival per consumer warpgroup
-    for (int s = 0; s < A_STAGES; ++s) { mbar_init(afull(s), 1); mbar_init(aempty(s), 2); }
-    for (int s = 0; s < 2; ++s) { mbar_init(bfull(s), 1); mbar_init(bempty(s), 2); }
+    for (int s = 0; s < A_STAGES; ++s) { mbar_init(sm.afull(s), 1); mbar_init(sm.aempty(s), 2); }
+    for (int s = 0; s < 2; ++s) { mbar_init(sm.bfull(s), 1); mbar_init(sm.bempty(s), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -143,25 +149,19 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmF1, const __grid_constant__
       int stage = 0; uint32_t phase = 0;
       int bsel = 0; uint32_t bphase = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const int per_img = tiles_per_par * S2 * S2;
-        const int img = tile / per_img;
-        int t = tile - img * per_img;
-        const int par = t / tiles_per_par;
-        t -= par * tiles_per_par;
-        const int py = par / S2, px = par % S2;
-        const int y0 = (t / p.tiles_x) * TH * S2, x0 = (t % p.tiles_x) * TW * S2;
+        const CorrTile t = corr_tile<R, S2>(p, tiles_per_par, tile);
         // f1 tile (MMA B operand): resident for the whole tile, double-buffered across tiles
-        mbar_wait(bempty(bsel), bphase ^ 1);
-        mbar_expect_tx(bfull(bsel), b_tile_bytes);
+        mbar_wait(sm.bempty(bsel), bphase ^ 1);
+        mbar_expect_tx(sm.bfull(bsel), b_tile_bytes);
         for (int kc = 0; kc < p.kch; ++kc)
-          tma_load_4d(b_buf + bsel * MAX_KCH * B_BYTES + kc * B_BYTES, &tmF1, bfull(bsel), kc * KC, x0 + px, y0 + py, img);
+          tma_load_4d(sm.b_buf + bsel * MAX_KCH * B_BYTES + kc * B_BYTES, &tmF1, sm.bfull(bsel), kc * KC, t.x0 + t.px, t.y0 + t.py, t.img);
         // f2 neighbourhood blocks (MMA A operand): 4 rows x 32 columns of same-parity pixels each
         for (int b = 0; b < NBLK; ++b) {
           for (int kc = 0; kc < p.kch; ++kc) {
-            mbar_wait(aempty(stage), phase ^ 1);
-            mbar_expect_tx(afull(stage), A_BYTES);
-            tma_load_4d(a_ring + stage * A_BYTES, &tmF2, afull(stage), kc * KC, x0 + px - R * S2,
-                        y0 + py + (4 * b - R) * S2, img);
+            mbar_wait(sm.aempty(stage), phase ^ 1);
+            mbar_expect_tx(sm.afull(stage), A_BYTES);
+            tma_load_4d(sm.a_ring + stage * A_BYTES, &tmF2, sm.afull(stage), kc * KC, t.x0 + t.px - R * S2,
+                        t.y0 + t.py + (4 * b - R) * S2, t.img);
             if (++stage == A_STAGES) { stage = 0; phase ^= 1; }
           }
         }
@@ -169,8 +169,8 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmF1, const __grid_constant__
       }
     }
   } else if (warp >= 4) {
-    if (p.f16) corr_consumer<R, S2, true>(p, a_ring, b_buf, bars, (warp - 4) >> 2);
-    else corr_consumer<R, S2, false>(p, a_ring, b_buf, bars, (warp - 4) >> 2);
+    if (p.f16) corr_consumer<R, S2, true>(p, sm, (warp - 4) >> 2);
+    else corr_consumer<R, S2, false>(p, sm, (warp - 4) >> 2);
   }
 }
 
@@ -193,7 +193,7 @@ int launch(const vps_tensor* f1, const vps_tensor* f2, const vps_tensor* out, in
       !vps::encode_nhwc(&tm2, *f2, type, KC, 32 * S2, 4 * S2, S2, S2, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                         "correlation_tc: encode f2"))
     return VPS_E_CUDA;
-  const int smem = A_STAGES * A_BYTES + 2 * MAX_KCH * B_BYTES + 1024 + 8 * (2 * A_STAGES + 12);
+  const int smem = (int)corr_smem(0).smem;
   auto kern = corr_tc_kernel<R, S2>;
   static bool attr_set = false;
   if (!attr_set) {
