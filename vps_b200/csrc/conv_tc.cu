@@ -43,6 +43,22 @@ __host__ __device__ __forceinline__ Ring tc_ring(uint32_t base, const ConvTcPara
   return rg;
 }
 
+// The K walk of a tile, which every role follows: bk channels of one filter tap per K step, chunk-major and tap-minor (a
+// chunk's taps in Tap order).  Halo mode: one A item per chunk feeds `rounds` B barrier rounds, of a filter row each (rowg)
+// or of one tap.  Flat mode: the tile's `steps` K steps fill ring slots of gsub steps, the last slot possibly fewer.  A step
+// of the last chunk has nk_last K16 slabs (bk = 64), the others 4.
+struct TcWalk {
+  const ConvTcParams& p;
+  __host__ __device__ __forceinline__ int chunks() const { return p.cin_chunks; }
+  __host__ __device__ __forceinline__ int taps() const { return p.kh * p.kw; }
+  __host__ __device__ __forceinline__ int rounds() const { return p.rowg ? p.kh : p.kh * p.kw; }
+  __host__ __device__ __forceinline__ int steps() const { return p.cin_chunks * p.kh * p.kw; }
+  __host__ __device__ __forceinline__ int slot_steps(int q0) const { return min(p.gsub, steps() - q0); }
+  __device__ __forceinline__ int chunk_nk(int cc) const { return cc == p.cin_chunks - 1 ? p.nk_last : 4; }
+  __device__ __forceinline__ int step_nk(int q) const { return q >= steps() - taps() ? p.nk_last : 4; }
+};
+__host__ __device__ __forceinline__ TcWalk tc_walk(const ConvTcParams& p) { return {p}; }
+
 // ---------------------------------------------------------------- TMA producer (warp 0)
 // The loop runs warp-uniformly and picks the issuing lane with elect.sync: code under `if (lane == 0)` is divergent to the
 // compiler, which then wraps every TMA instruction in a uniformity loop.  In halo mode one barrier round covers a whole
@@ -53,31 +69,30 @@ template <bool ROWG>
 __device__ __forceinline__ void producer_halo(const ConvTcParams& p, const Ring& rg, const CUtensorMap* tmA,
                                               const CUtensorMap* tmB0, const CUtensorMap* tmB1, const CUtensorMap* tmB2,
                                               const CUtensorMap* tmB3) {
-  const int bk = p.bk, kw = p.kw, cin_chunks = p.cin_chunks, a_stages = p.a_stages, b_stages = p.b_stages;
-  const int ngrp = ROWG ? p.kh : p.kh * p.kw;
+  const int bk = p.bk, kw = p.kw, a_stages = p.a_stages, b_stages = p.b_stages;
+  const TcWalk walk = tc_walk(p);
   const uint32_t a_box_bytes = (uint32_t)p.a_box_bytes;
-  int as = 0, bs = 0;
-  uint32_t aphase = 0, bphase = 0;
+  RingPos ap, bp;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const TileCoord t = tile_coord(p, tile);
     const int x_base = t.tx * p.tw - p.pw_[t.prob];
     const int y_base = t.ty * p.th - p.ph_[t.prob];
     const int n0 = t.n_idx * p.block_n;
     const CUtensorMap* tmB = t.prob == 0 ? tmB0 : (t.prob == 1 ? tmB1 : (t.prob == 2 ? tmB2 : tmB3));
-    for (int cc = 0; cc < cin_chunks; ++cc) {
-      mbar_wait(rg.aempty(as), aphase ^ 1);
+    for (int cc = 0; cc < walk.chunks(); ++cc) {
+      ap.wait_empty(rg.aempty(ap.slot));
       if (elect_one()) {
-        mbar_expect_tx(rg.afull(as), a_box_bytes);
-        tma_load_4d(rg.a_base + as * rg.a_stage_bytes, tmA, rg.afull(as), cc * bk, x_base, y_base, t.img);
+        mbar_expect_tx(rg.afull(ap.slot), a_box_bytes);
+        tma_load_4d(rg.a_base + ap.slot * rg.a_stage_bytes, tmA, rg.afull(ap.slot), cc * bk, x_base, y_base, t.img);
       }
-      if (++as == a_stages) { as = 0; aphase ^= 1; }
-      for (int g = 0; g < ngrp; ++g) {
-        mbar_wait(rg.bempty(bs), bphase ^ 1);
+      ap.next(a_stages);
+      for (int g = 0; g < walk.rounds(); ++g) {
+        bp.wait_empty(rg.bempty(bp.slot));
         if (elect_one()) {
-          mbar_expect_tx(rg.bfull(bs), rg.b_stage_bytes);
-          tma_load_3d(rg.b_base + bs * rg.b_stage_bytes, tmB, rg.bfull(bs), cc * bk, n0, ROWG ? g * kw : g);
+          mbar_expect_tx(rg.bfull(bp.slot), rg.b_stage_bytes);
+          tma_load_3d(rg.b_base + bp.slot * rg.b_stage_bytes, tmB, rg.bfull(bp.slot), cc * bk, n0, ROWG ? g * kw : g);
         }
-        if (++bs == b_stages) { bs = 0; bphase ^= 1; }
+        bp.next(b_stages);
       }
     }
   }
@@ -88,33 +103,34 @@ __device__ __forceinline__ void producer_halo(const ConvTcParams& p, const Ring&
 __device__ __forceinline__ void producer_flat(const ConvTcParams& p, const Ring& rg, const CUtensorMap* tmA,
                                               const CUtensorMap* tmB0, const CUtensorMap* tmB1, const CUtensorMap* tmB2,
                                               const CUtensorMap* tmB3) {
-  const int bk = p.bk, kw = p.kw, kh = p.kh, stages = p.a_stages, G = p.gsub;
-  const int T = p.cin_chunks * kh * kw;
+  const int bk = p.bk, stages = p.a_stages;
+  const TcWalk walk = tc_walk(p);
   const uint32_t a_box_bytes = (uint32_t)p.a_box_bytes;
   const uint32_t b_tile_bytes = (uint32_t)p.block_n * (uint32_t)bk * 2u;
-  int st = 0;
-  uint32_t phase = 0;
+  RingPos sp;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const TileCoord t = tile_coord(p, tile);
     const int x_base = t.tx * p.tw * p.sw - p.pw_[t.prob];
     const int y_base = t.ty * p.th * p.sh - p.ph_[t.prob];
     const int n0 = t.n_idx * p.block_n;
     const CUtensorMap* tmB = t.prob == 0 ? tmB0 : (t.prob == 1 ? tmB1 : (t.prob == 2 ? tmB2 : tmB3));
-    int cc = 0, r = 0, sx = 0;
-    for (int q0 = 0; q0 < T; q0 += G) {
-      const int cnt = min(G, T - q0);
-      mbar_wait(rg.aempty(st), phase ^ 1);
-      const uint32_t a_slot = rg.a_base + st * rg.a_stage_bytes, b_slot = rg.b_base + st * rg.b_stage_bytes;
-      if (elect_one()) mbar_expect_tx(rg.afull(st), (uint32_t)cnt * (a_box_bytes + b_tile_bytes));
+    int cc = 0;
+    Tap tap;
+    for (int q0 = 0; q0 < walk.steps(); q0 += p.gsub) {
+      const int cnt = walk.slot_steps(q0);
+      sp.wait_empty(rg.aempty(sp.slot));
+      const uint32_t a_slot = rg.a_base + sp.slot * rg.a_stage_bytes, b_slot = rg.b_base + sp.slot * rg.b_stage_bytes;
+      if (elect_one()) mbar_expect_tx(rg.afull(sp.slot), (uint32_t)cnt * (a_box_bytes + b_tile_bytes));
       __syncwarp();
       for (int j = 0; j < cnt; ++j) {
         if (elect_one()) {
-          tma_load_4d(a_slot + j * a_box_bytes, tmA, rg.afull(st), cc * bk, x_base + sx, y_base + r, t.img);
-          tma_load_3d(b_slot + j * b_tile_bytes, tmB, rg.afull(st), cc * bk, n0, r * kw + sx);
+          tma_load_4d(a_slot + j * a_box_bytes, tmA, rg.afull(sp.slot), cc * bk, x_base + tap.s, y_base + tap.r, t.img);
+          tma_load_3d(b_slot + j * b_tile_bytes, tmB, rg.afull(sp.slot), cc * bk, n0, tap.k);
         }
-        if (++sx == kw) { sx = 0; if (++r == kh) { r = 0; ++cc; } }
+        tap.next(p.kw);
+        if (tap.r == p.kh) { tap = Tap(); ++cc; }
       }
-      if (++st == stages) { st = 0; phase ^= 1; }
+      sp.next(stages);
     }
   }
 }
@@ -152,30 +168,29 @@ template <int N, bool BK64>
 __device__ __forceinline__ void consumer_tc(const ConvTcParams& p, const Ring& rg, int wg) {
   constexpr uint32_t row_bytes = BK64 ? 128u : 32u;
   const bool leader = (threadIdx.x & 127) == 0;
-  const int kw = p.kw, cin_chunks = p.cin_chunks, nk_last = p.nk_last;
+  const int kw = p.kw;
+  const TcWalk walk = tc_walk(p);
   const uint32_t tap_b_bytes = (uint32_t)N * row_bytes;
   const uint64_t b_hi = desc_hi(row_bytes, 8u * row_bytes);
   float d[N / 2];
-  int as = 0, bs = 0;
-  uint32_t aphase = 0, bphase = 0;
+  RingPos ap, bp;
   Release rel;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     uint32_t accumulate = 0;
     if (p.halo) {
       // the 8 rows of an MMA row group are 8 pixels of one halo row; this warpgroup's 64 pixels start 8 halo rows down
-      const int ngrp = p.rowg ? p.kh : p.kh * kw;
       const uint32_t halo_pitch = (uint32_t)p.halo_w * row_bytes;
       const uint64_t a_hi = desc_hi(row_bytes, halo_pitch);
-      for (int cc = 0; cc < cin_chunks; ++cc) {
-        const int nk = cc == cin_chunks - 1 ? nk_last : 4;
-        mbar_wait(rg.afull(as), aphase);
-        uint32_t a_row = rg.a_base + as * rg.a_stage_bytes + (uint32_t)wg * 8u * halo_pitch, a_tap = a_row;
-        const int a_cur = as;
+      for (int cc = 0; cc < walk.chunks(); ++cc) {
+        const int nk = walk.chunk_nk(cc);
+        ap.wait_full(rg.afull(ap.slot));
+        uint32_t a_row = rg.a_base + ap.slot * rg.a_stage_bytes + (uint32_t)wg * 8u * halo_pitch, a_tap = a_row;
+        const int a_cur = ap.slot;
         int sx = 0;
-        if (++as == p.a_stages) { as = 0; aphase ^= 1; }
-        for (int g = 0; g < ngrp; ++g) {
-          mbar_wait(rg.bfull(bs), bphase);
-          const uint32_t b_addr = rg.b_base + bs * rg.b_stage_bytes;
+        ap.next(p.a_stages);
+        for (int g = 0; g < walk.rounds(); ++g) {
+          bp.wait_full(rg.bfull(bp.slot));
+          const uint32_t b_addr = rg.b_base + bp.slot * rg.b_stage_bytes;
           wg::fence();
           if (p.rowg) {      // the kw taps of filter row g: A start moves one pixel (row_bytes) per tap
             for (int j = 0; j < kw; ++j) issue_tap<N, BK64>(d, a_hi, b_hi, a_row + j * row_bytes, b_addr + j * tap_b_bytes, nk, accumulate);
@@ -185,9 +200,9 @@ __device__ __forceinline__ void consumer_tc(const ConvTcParams& p, const Ring& r
           wg::commit();
           wg::wait<1>();
           rel.flush(rg, leader);
-          rel.b = bs;
-          if (g == ngrp - 1) rel.a = a_cur;
-          if (++bs == p.b_stages) { bs = 0; bphase ^= 1; }
+          rel.b = bp.slot;
+          if (g == walk.rounds() - 1) rel.a = a_cur;
+          bp.next(p.b_stages);
           if (p.rowg) {
             a_row += halo_pitch;
           } else {          // next tap: one pixel to the right, or the start of the next halo row
@@ -198,24 +213,21 @@ __device__ __forceinline__ void consumer_tc(const ConvTcParams& p, const Ring& r
       }
     } else {
       // flat mode: gsub K steps per ring slot, operands of both kinds on the slot's `afull` barrier
-      const int ntaps = p.kh * kw, G = p.gsub;
-      const int T = cin_chunks * ntaps, q_last = T - ntaps;
       const uint32_t a_box_bytes = (uint32_t)p.a_box_bytes;
       const uint64_t a_hi = desc_hi(row_bytes, 8u * row_bytes);
-      for (int q0 = 0; q0 < T; q0 += G) {
-        const int cnt = min(G, T - q0);
-        mbar_wait(rg.afull(as), aphase);
-        const uint32_t a_slot = rg.a_base + as * rg.a_stage_bytes + (uint32_t)wg * 64u * row_bytes;
-        const uint32_t b_slot = rg.b_base + as * rg.b_stage_bytes;
+      for (int q0 = 0; q0 < walk.steps(); q0 += p.gsub) {
+        const int cnt = walk.slot_steps(q0);
+        ap.wait_full(rg.afull(ap.slot));
+        const uint32_t a_slot = rg.a_base + ap.slot * rg.a_stage_bytes + (uint32_t)wg * 64u * row_bytes;
+        const uint32_t b_slot = rg.b_base + ap.slot * rg.b_stage_bytes;
         wg::fence();
         for (int j = 0; j < cnt; ++j)
-          issue_tap<N, BK64>(d, a_hi, b_hi, a_slot + j * a_box_bytes, b_slot + j * tap_b_bytes, q0 + j >= q_last ? nk_last : 4,
-                             accumulate);
+          issue_tap<N, BK64>(d, a_hi, b_hi, a_slot + j * a_box_bytes, b_slot + j * tap_b_bytes, walk.step_nk(q0 + j), accumulate);
         wg::commit();
         wg::wait<1>();
         rel.flush(rg, leader);
-        rel.a = as;
-        if (++as == p.a_stages) { as = 0; aphase ^= 1; }
+        rel.a = ap.slot;
+        ap.next(p.a_stages);
       }
     }
     wg::wait<0>();
@@ -247,10 +259,10 @@ conv_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);     // warp-uniform role index (wgmma issue is not treated as divergent)
   const int lane = threadIdx.x & 31;
 
-  // barrier slots (8 B each): afull, aempty, bfull, bempty [MAX_STAGES each]; full = one TMA arrival, empty = one arrival
-  // per consumer warpgroup
+  // full = one TMA arrival, empty = one arrival per consumer warpgroup
   if (warp == 0) {
-    mbar_init(rg.bar_base + 8u * lane, (lane >> 3) & 1 ? 2 : 1);
+    if (lane < MAX_STAGES) { mbar_init(rg.afull(lane), 1); mbar_init(rg.aempty(lane), 2); }
+    else if (lane < 2 * MAX_STAGES) { mbar_init(rg.bfull(lane - MAX_STAGES), 1); mbar_init(rg.bempty(lane - MAX_STAGES), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (threadIdx.x == 32) {
@@ -289,9 +301,9 @@ constexpr int DCN_MAX_N = 128;
 
 __device__ __forceinline__ void dcn_gather_loop(const ConvTcParams& p, const DcnParams<__nv_bfloat16>& d, const Ring& rg,
                                                 uint32_t setup_base, int gtid) {
-  const int stages = p.a_stages, cin_chunks = p.cin_chunks;
-  int st = 0;
-  uint32_t phase = 0;
+  const int stages = p.a_stages;
+  const TcWalk walk = tc_walk(p);
+  RingPos sp;
   const int j = gtid & 7;                    // 16-byte channel chunk of the 128-byte row
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const TileCoord tc = tile_coord(p, tile);
@@ -304,11 +316,11 @@ __device__ __forceinline__ void dcn_gather_loop(const ConvTcParams& p, const Dcn
     }
     asm volatile("bar.sync 1, %0;" ::"n"(32 * DCN_GATHER_WARPS) : "memory");
     // ---- K steps: chunk-major, tap-minor
-    for (int cc = 0; cc < cin_chunks; ++cc) {
+    for (int cc = 0; cc < walk.chunks(); ++cc) {
       const __nv_bfloat16* xc = d.x + cc * 64 + j * 8;
-      for (int k = 0; k < 9; ++k) {
-        mbar_wait(rg.aempty(st), phase ^ 1);
-        const uint32_t a_slot = rg.a_base + st * rg.a_stage_bytes;
+      for (int k = 0; k < walk.taps(); ++k) {
+        sp.wait_empty(rg.aempty(sp.slot));
+        const uint32_t a_slot = rg.a_base + sp.slot * rg.a_stage_bytes;
         constexpr int ROWS_PER_PASS = 32 * DCN_GATHER_WARPS / 8;       // 8 lanes (16-byte chunks) per pixel row
         for (int r = gtid >> 3; r < BLOCK_M; r += ROWS_PER_PASS) {
           const uint32_t sa = setup_base + (uint32_t)(k * BLOCK_M + r) * 32u;
@@ -345,8 +357,8 @@ __device__ __forceinline__ void dcn_gather_loop(const ConvTcParams& p, const Dcn
           asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(da), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]), "r"(pk[3]) : "memory");
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> tensor-core reads
-        mbar_arrive(rg.afull(st));
-        if (++st == stages) { st = 0; phase ^= 1; }
+        mbar_arrive(rg.afull(sp.slot));
+        sp.next(stages);
       }
     }
     asm volatile("bar.sync 1, %0;" ::"n"(32 * DCN_GATHER_WARPS) : "memory");   // set-up cache is rewritten next tile
@@ -376,19 +388,18 @@ dcn_igemm_tc_kernel(const __grid_constant__ CUtensorMap tmB, const ConvTcParams 
   } else {
     if (warp == 0) {
       // weight producer: one {64 ch, block_n, 1 tap} box per K step, completing on the step's `afull` barrier
-      const int stages = p.a_stages;
-      int st = 0;
-      uint32_t phase = 0;
+      const TcWalk walk = tc_walk(p);
+      RingPos sp;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         const int n0 = tile_coord(p, tile).n_idx * p.block_n;
-        for (int cc = 0; cc < p.cin_chunks; ++cc) {
-          for (int k = 0; k < 9; ++k) {
-            mbar_wait(rg.aempty(st), phase ^ 1);
+        for (int cc = 0; cc < walk.chunks(); ++cc) {
+          for (int k = 0; k < walk.taps(); ++k) {
+            sp.wait_empty(rg.aempty(sp.slot));
             if (elect_one()) {
-              mbar_expect_tx(rg.afull(st), rg.b_stage_bytes);
-              tma_load_3d(rg.b_base + st * rg.b_stage_bytes, &tmB, rg.afull(st), cc * 64, n0, k);
+              mbar_expect_tx(rg.afull(sp.slot), rg.b_stage_bytes);
+              tma_load_3d(rg.b_base + sp.slot * rg.b_stage_bytes, &tmB, rg.afull(sp.slot), cc * 64, n0, k);
             }
-            if (++st == stages) { st = 0; phase ^= 1; }
+            sp.next(p.a_stages);
           }
         }
       }
@@ -507,15 +518,14 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
   set_tiles(p, a, nprob, tw, th, block_n, bk);
   // halo mode: one B ring slot = the kw taps of a filter row when that fits (<= 48 KB) -- one barrier round per row
   p.rowg = (halo && a->kw > 1 && a->kw * block_n * bk * 2 <= 48 * 1024) ? 1 : 0;
-  p.nk_last = bk == 64 ? (a->cin - (p.cin_chunks - 1) * 64 + 15) / 16 : 1;
   // flat mode: gsub consecutive K steps share a ring slot (<= 48 KB of operands per barrier round, at most 4 steps)
   p.gsub = 1;
   if (!halo) {
     const int step_bytes = p.a_box_bytes + block_n * bk * 2;
     int g = (48 * 1024) / step_bytes;
-    const int T = p.cin_chunks * a->kh * a->kw;
+    const int steps = tc_walk(p).steps();
     if (g > 4) g = 4;
-    if (g > T) g = T;
+    if (g > steps) g = steps;
     if (g < 1) g = 1;
     p.gsub = g;
     p.a_stage_bytes = g * p.a_box_bytes;
@@ -571,7 +581,7 @@ extern "C" int vps_deform_conv_tc(const vps_tensor* x, const vps_tensor* offset,
   // weight rows past cout_pad are TMA zero fill
   const int tw = patch_tw(x->h, x->w, BLOCK_M, 1, 1);
   set_tiles(p, &a, 1, tw, BLOCK_M / tw, cout_pad <= 64 ? 64 : DCN_MAX_N, 64);
-  p.gsub = 1; p.nk_last = 4;
+  p.gsub = 1;
   p.a_box_bytes = BLOCK_M * 128; p.a_stage_bytes = p.a_box_bytes;
   int stages = (200 * 1024 - dcn_setup_bytes(BLOCK_M)) / (p.a_stage_bytes + (int)tc_ring(0, p, true).b_stage_bytes);
   if (stages > MAX_STAGES) stages = MAX_STAGES;

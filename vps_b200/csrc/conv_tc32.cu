@@ -121,39 +121,47 @@ __host__ __device__ __forceinline__ Ring32 ring32(uint32_t base, const ConvTcPar
   return rg;
 }
 
+// The K walk of a tile, which every role follows: T32_KC channels of one filter tap per step, chunk-major and tap-minor
+// (a loop over chunks around a loop over Tap).  An A item -- one converted or sampled box -- feeds all taps of a chunk in
+// halo mode and one step otherwise.  The second K16 slab of a step is padding only in the last chunk, when p.nk_last is 1.
+struct Tc32Walk {
+  int chunks, taps, kw;
+  bool halo;
+  __host__ __device__ __forceinline__ int steps() const { return chunks * taps; }
+  __host__ __device__ __forceinline__ int items() const { return chunks * (halo ? 1 : taps); }
+  __device__ __forceinline__ bool opens_item(int tap) const { return !halo || tap == 0; }
+};
+__host__ __device__ __forceinline__ Tc32Walk tc32_walk(const ConvTcParams& p) { return {p.cin_chunks, p.kh * p.kw, p.kw, p.halo != 0}; }
+
 // ---------------------------------------------------------------- warp 0: TMA producer
 __device__ __forceinline__ void producer32(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, const CUtensorMap* tmA,
                                            const CUtensorMap* tmB) {
-  const int ntaps = p.kh * p.kw, kw = p.kw;
-  const bool halo = p.halo != 0;
+  const Tc32Walk walk = tc32_walk(p);
   const uint32_t a_box_bytes = (uint32_t)p.a_box_bytes, b_bytes = (uint32_t)T32_PLANES * (uint32_t)e.b_plane_bytes;
   const int bn = p.block_n;
-  int ss = 0, bs = 0;
-  uint32_t sphase = 0, bphase = 0;
+  RingPos sp, bp;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const TileCoord t = tile_coord(p, tile);
     const int x_base = t.tx * p.tw * p.sw - p.pw_[t.prob];
     const int y_base = t.ty * p.th * p.sh - p.ph_[t.prob];
     const int n0 = t.n_idx * bn;
-    for (int cc = 0; cc < p.cin_chunks; ++cc) {
-      int r = 0, s = 0;
-      for (int tap = 0; tap < ntaps; ++tap) {
-        if (!e.dcn && (!halo || tap == 0)) {
-          mbar_wait(rg.sempty(ss), sphase ^ 1);
+    for (int cc = 0; cc < walk.chunks; ++cc) {
+      for (Tap tap; tap.k < walk.taps; tap.next(walk.kw)) {
+        if (!e.dcn && walk.opens_item(tap.k)) {
+          sp.wait_empty(rg.sempty(sp.slot));
           if (elect_one()) {
-            mbar_expect_tx(rg.sfull(ss), a_box_bytes);
-            tma_load_4d(rg.s_base + ss * rg.s_bytes, tmA, rg.sfull(ss), cc * T32_KC, halo ? x_base : x_base + s,
-                        halo ? y_base : y_base + r, t.img);
+            mbar_expect_tx(rg.sfull(sp.slot), a_box_bytes);
+            tma_load_4d(rg.s_base + sp.slot * rg.s_bytes, tmA, rg.sfull(sp.slot), cc * T32_KC,
+                        walk.halo ? x_base : x_base + tap.s, walk.halo ? y_base : y_base + tap.r, t.img);
           }
-          if (++ss == T32_STAGE_SLOTS) { ss = 0; sphase ^= 1; }
+          sp.next(T32_STAGE_SLOTS);
         }
-        mbar_wait(rg.bempty(bs), bphase ^ 1);
+        bp.wait_empty(rg.bempty(bp.slot));
         if (elect_one()) {     // both weight planes of this (tap, chunk) in one 5-D box
-          mbar_expect_tx(rg.bfull(bs), b_bytes);
-          tma_load_5d(rg.b_base + bs * rg.b_bytes, tmB, rg.bfull(bs), cc * T32_KC, n0, tap, t.prob, 0);
+          mbar_expect_tx(rg.bfull(bp.slot), b_bytes);
+          tma_load_5d(rg.b_base + bp.slot * rg.b_bytes, tmB, rg.bfull(bp.slot), cc * T32_KC, n0, tap.k, t.prob, 0);
         }
-        if (++bs == p.b_stages) { bs = 0; bphase ^= 1; }
-        if (++s == kw) { s = 0; ++r; }
+        bp.next(p.b_stages);
       }
     }
   }
@@ -161,18 +169,16 @@ __device__ __forceinline__ void producer32(const ConvTcParams& p, const Tc32Extr
 
 // ---------------------------------------------------------------- warps 1..3: fp32 box -> fp16 main / correction operand planes
 __device__ __forceinline__ void converter32(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, int ctid, int nthreads) {
-  const int ntaps = p.kh * p.kw;
-  const int items_per_tile = p.cin_chunks * (p.halo ? 1 : ntaps);
+  const int items_per_tile = tc32_walk(p).items();
   const int tasks = e.rows * 4;                       // 8 channels (two 16-byte fp32 chunks) per task
-  int ss = 0, as = 0;
-  uint32_t sphase = 0, aphase = 0;
+  RingPos sp, ap;
   bool over = false;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     for (int it = 0; it < items_per_tile; ++it) {
-      mbar_wait(rg.sfull(ss), sphase);
-      mbar_wait(rg.pempty(as), aphase ^ 1);
-      const uint32_t src = rg.s_base + ss * rg.s_bytes;
-      const uint32_t dst = rg.a_base + as * rg.a_bytes;
+      sp.wait_full(rg.sfull(sp.slot));
+      ap.wait_empty(rg.pempty(ap.slot));
+      const uint32_t src = rg.s_base + sp.slot * rg.s_bytes;
+      const uint32_t dst = rg.a_base + ap.slot * rg.a_bytes;
       for (int task = ctid; task < tasks; task += nthreads) {
         const int r = task >> 2, j = task & 3;
         // staging rows are 128 bytes, SWIZZLE_128B (written by TMA): 16-byte chunk c of row r sits at chunk c ^ (r & 7)
@@ -192,11 +198,11 @@ __device__ __forceinline__ void converter32(const ConvTcParams& p, const Tc32Ext
         asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(pm), "r"(hp[0]), "r"(hp[1]), "r"(hp[2]), "r"(hp[3]) : "memory");
         asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(pl), "r"(lp[0]), "r"(lp[1]), "r"(lp[2]), "r"(lp[3]) : "memory");
       }
-      mbar_arrive(rg.sempty(ss));                                        // staging slot may be refilled
+      mbar_arrive(rg.sempty(sp.slot));                                   // staging slot may be refilled
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // generic-proxy writes -> tensor-core reads
-      mbar_arrive(rg.pfull(as));
-      if (++ss == T32_STAGE_SLOTS) { ss = 0; sphase ^= 1; }
-      if (++as == p.a_stages) { as = 0; aphase ^= 1; }
+      mbar_arrive(rg.pfull(ap.slot));
+      sp.next(T32_STAGE_SLOTS);
+      ap.next(p.a_stages);
     }
   }
   if (over) atomicAdd(&g_tc32_overflow, 1u);
@@ -216,9 +222,9 @@ __device__ __forceinline__ void dcn_gather32(const ConvTcParams& p, const Tc32Ex
   const int lane = gtid & 31;
   const int j = lane & 3;                    // 8-channel group of the 32-channel chunk
   const int rlog = e.rows == 128 ? 7 : 6, ulog = rlog - 3;
-  const int steps_per_tile = p.cin_chunks * 9;
+  const Tc32Walk walk = tc32_walk(p);
+  const int steps_per_tile = walk.steps();
   const uint32_t units_per_tile = (uint32_t)steps_per_tile << ulog;   // a unit = 8 rows (pixels) x 32 channels of one K step
-  const uint32_t a_stages = (uint32_t)p.a_stages;
   uint32_t step_base = 0;                    // K steps of the tiles this CTA has finished
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const TileCoord t = tile_coord(p, tile);
@@ -238,11 +244,10 @@ __device__ __forceinline__ void dcn_gather32(const ConvTcParams& p, const Tc32Ex
       u = __shfl_sync(0xffffffffu, u, 0);
       if (u >= units_per_tile) break;
       const uint32_t step = u >> ulog, part = u & ((1u << ulog) - 1u);
-      const uint32_t cc = step / 9u, k = step - cc * 9u;
-      const uint32_t sg = step_base + step;             // K step counted over all tiles of this CTA -> ring slot and its use count
-      const uint32_t use = sg / a_stages, as = sg - use * a_stages;
-      mbar_wait(rg.pempty((int)as), (use & 1u) ^ 1u);
-      const uint32_t dst = rg.a_base + as * rg.a_bytes;
+      const uint32_t cc = step / (uint32_t)walk.taps, k = step - cc * (uint32_t)walk.taps;
+      const RingPos ap = RingPos::at(step_base + step, (uint32_t)p.a_stages);   // K step counted over this CTA's tiles
+      ap.wait_empty(rg.pempty(ap.slot));
+      const uint32_t dst = rg.a_base + ap.slot * rg.a_bytes;
       const int r = (int)(part * 8u) + (lane >> 2);
       const float* xc = d.x + cc * T32_KC + j * 8;
       {
@@ -278,7 +283,7 @@ __device__ __forceinline__ void dcn_gather32(const ConvTcParams& p, const Tc32Ex
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy writes -> tensor-core reads
       __syncwarp();
-      if (lane == 0) mbar_arrive(rg.pfull((int)as));                   // e.rows / 8 warp-units complete a K step's operand planes
+      if (lane == 0) mbar_arrive(rg.pfull(ap.slot));                   // e.rows / 8 warp-units complete a K step's operand planes
     }
     step_base += (uint32_t)steps_per_tile;
     asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory");      // the set-up table and the unit counter are rewritten for the next tile
@@ -364,6 +369,8 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
   const uint32_t box = rg.e_base + (uint32_t)wg * (64u * N * 4u), bias_s = rg.bias_base + (uint32_t)wg * (N * 4u);
   const uint32_t rbar = rg.rfull(wg);
   uint32_t rphase = 0;
+  // The K walk is Tc32Walk's, spelled out: the same expressions through Tc32Walk's members make ptxas allocate 4 more
+  // registers to the 640-thread TMA-epilogue kernel.
   const bool halo = p.halo != 0;
   const int ntaps = p.kh * p.kw, kw = p.kw, last_cc = p.cin_chunks - 1;
   const uint32_t a_pitch = halo ? (uint32_t)p.halo_w * 64u : 512u;      // byte distance of the A planes' 8-row groups
@@ -372,8 +379,7 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
   const uint32_t a_wg = halo ? (uint32_t)(row0 >> 3) * a_pitch : (uint32_t)row0 * 64u;
   const uint32_t plane = (uint32_t)e.plane_bytes, b_plane = (uint32_t)e.b_plane_bytes;
   float acc[N / 2], sum[N / 2];
-  int as = 0, bs = 0;
-  uint32_t aphase = 0, bphase = 0;
+  RingPos ap, bp;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     float bias_v = 0.f;
     if (epi_tma) {        // this thread's bias value of the tile: loaded now, written to shared memory in the epilogue
@@ -385,15 +391,14 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
     for (int cc = 0; cc <= last_cc; ++cc) {
       const bool two = cc != last_cc || p.nk_last > 1;
       uint32_t a_item = 0;
-      int r = 0, s = 0;
-      for (int tap = 0; tap < ntaps; ++tap) {
-        if (!halo || tap == 0) {
-          mbar_wait(rg.pfull(as), aphase);
-          a_item = rg.a_base + as * rg.a_bytes + a_wg;
+      for (Tap tap; tap.k < ntaps; tap.next(kw)) {
+        if (!halo || tap.k == 0) {
+          ap.wait_full(rg.pfull(ap.slot));
+          a_item = rg.a_base + ap.slot * rg.a_bytes + a_wg;
         }
-        mbar_wait(rg.bfull(bs), bphase);
-        const uint32_t a_addr = halo ? a_item + (uint32_t)r * a_pitch + (uint32_t)s * 64u : a_item;
-        const uint32_t b_addr = rg.b_base + bs * rg.b_bytes + b_off;
+        bp.wait_full(rg.bfull(bp.slot));
+        const uint32_t a_addr = halo ? a_item + (uint32_t)tap.r * a_pitch + (uint32_t)tap.s * 64u : a_item;
+        const uint32_t b_addr = rg.b_base + bp.slot * rg.b_bytes + b_off;
         const uint64_t A = desc_at(a_hi, a_addr), A2 = desc_at(a_hi, a_addr + plane);
         const uint64_t B = desc_at(b_hi, b_addr), B2 = desc_at(b_hi, b_addr + b_plane);
         wg::fence();
@@ -414,11 +419,11 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
         wg::fence_regs(acc);
 #pragma unroll
         for (int i = 0; i < N / 2; ++i) sum[i] += acc[i];
-        const bool item_done = !halo || tap == ntaps - 1;
+        const bool item_done = !halo || tap.k == ntaps - 1;
         if (leader) {
-          mbar_arrive(rg.bempty(bs));
-          if (item_done) mbar_arrive(rg.pempty(as));
-          if (epi_tma && p.res && cc == 0 && tap == 0) {
+          mbar_arrive(rg.bempty(bp.slot));
+          if (item_done) mbar_arrive(rg.pempty(ap.slot));
+          if (epi_tma && p.res && cc == 0 && tap.k == 0) {
             asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
             const EpiBox eb = epi_box(p, tile, wg);
             if (eb.live) {
@@ -431,9 +436,8 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
             }
           }
         }
-        if (item_done && ++as == p.a_stages) { as = 0; aphase ^= 1; }
-        if (++bs == p.b_stages) { bs = 0; bphase ^= 1; }
-        if (++s == kw) { s = 0; ++r; }
+        ap.next(p.a_stages, item_done);
+        bp.next(p.b_stages);
       }
     }
     if (epi_tma) {
@@ -607,7 +611,6 @@ Tc32Plan tc32_tile(const vps_conv_args* a, int nprob, int nwg, int block_n) {
   const int tw = p.halo ? 8 : patch_tw(a->oh, a->ow, px, a->sh, a->sw);
   set_tiles(p, a, nprob, tw, px / tw, block_n, T32_KC);
   p.halo_w = tw + a->kw - 1;
-  p.nk_last = (a->cin - (p.cin_chunks - 1) * T32_KC + 15) / 16;
   p.a_stages = p.halo ? 2 : 3;
   g.e.rows = p.halo ? (p.th + a->kh - 1) * p.halo_w : px;
   p.a_box_bytes = g.e.rows * 128;
@@ -636,7 +639,6 @@ int tc32_plan(const vps_conv_args* a, int nprob, Tc32Plan& out) {
   const int sms = vps::num_sms();
   if (sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
   const int cout_pad = (a->cout + 15) / 16 * 16;
-  const int steps = (a->cin + T32_KC - 1) / T32_KC * a->kh * a->kw;
   double best = -1.0;
   for (int nwg = 2; nwg <= 4; nwg += 2) {
     for (int bn = 16; bn <= (nwg == 2 ? T32_MAX_N : T32_WIDE_MAX_N) && bn <= cout_pad; bn *= 2) {
@@ -648,7 +650,7 @@ int tc32_plan(const vps_conv_args* a, int nprob, Tc32Plan& out) {
       const double waves = (double)((tiles + sms - 1) / sms);
       const double conv = 2.0 * (g.p.halo ? (double)g.e.rows / (a->kh * a->kw) : (double)g.e.rows);
       const double step = fmax(fmax(300.0, 1.5 * nwg * bn), fmax((double)(bn * 64 * T32_PLANES) / 56.0, conv));
-      const double t = waves * ((double)steps * step + 40.0 * bn + 1500.0);
+      const double t = waves * ((double)tc32_walk(g.p).steps() * step + 40.0 * bn + 1500.0);
       if (best < 0 || t < best * 0.999) {
         best = t;
         out = g;
@@ -699,7 +701,6 @@ int dcn32_plan(const vps_conv_args* a, Tc32Plan& out) {
   const int sms = vps::num_sms();
   if (sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
   const int cout_pad = (a->cout + 15) / 16 * 16;
-  const int steps = a->cin / T32_KC * 9;
   double best = -1.0, best_units = 0.0;
   for (int split_n = 0; split_n <= 1; ++split_n) {
     const int rows = split_n ? 64 : 128;        // tile pixels: split-M or split-N
@@ -709,7 +710,7 @@ int dcn32_plan(const vps_conv_args* a, Tc32Plan& out) {
       if (block_n > cout_pad || cout_pad % block_n) continue;
       Tc32Plan g = {};
       set_tiles(g.p, a, 1, tw, rows / tw, block_n, T32_KC);
-      g.p.nk_last = 2; g.p.a_stages = 2;
+      g.p.a_stages = 2;
       g.e.rows = rows; g.e.plane_bytes = rows * 64; g.e.b_plane_bytes = block_n * 64; g.e.dcn = 1; g.e.dcn_split_n = split_n;
       const Ring32 rg = ring32(0, g.p, g.e, 2, false, true);
       const int bst = (DCN32_SMEM_MAX - (int)rg.smem) / (int)rg.b_bytes;
@@ -717,7 +718,7 @@ int dcn32_plan(const vps_conv_args* a, Tc32Plan& out) {
       const int64_t tiles = g.p.total_tiles;
       const double waves = (double)((tiles + sms - 1) / sms);
       const double step = fmax(fmax(rows / 8 * DCN32_UNIT_CLK, fmax(DCN32_STEP_CLK, 6.0 * bn)), rg.b_bytes / 56.0);
-      const double t = waves * ((double)steps * step + 40.0 * bn + 1500.0), units = waves * rows;
+      const double t = waves * ((double)tc32_walk(g.p).steps() * step + 40.0 * bn + 1500.0), units = waves * rows;
       if (best < 0 || t < best * 0.999 || (t <= best * 1.001 && units < best_units)) {
         best = t; best_units = units;
         g.p.b_stages = bst > 3 ? 3 : bst;

@@ -225,7 +225,31 @@ __device__ __forceinline__ void dcn_setup_entry(const DcnParams<T>& d, uint32_t 
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sa + 16u), "r"(offs[0]), "r"(offs[1]), "r"(offs[2]), "r"(offs[3]) : "memory");
 }
 
-// ---------------------------------------------------------------- tile walk shared by the roles
+// ---------------------------------------------------------------- ring positions and the K walk shared by the roles
+// Position in a ring of `slots` mbarrier-guarded slots: the slot and the parity of its current use.  A reader waits for the
+// slot's full barrier at `phase`; a writer waits for its empty barrier at `phase ^ 1`, which the barrier's initial phase
+// satisfies on the first pass through the ring.
+struct RingPos {
+  int slot = 0;
+  uint32_t phase = 0;
+  // the position of use n (counted from 0)
+  __device__ __forceinline__ static RingPos at(uint32_t n, uint32_t slots) { return {(int)(n % slots), (n / slots) & 1u}; }
+  __device__ __forceinline__ void wait_full(uint32_t bar) const { mbar_wait(bar, phase); }
+  __device__ __forceinline__ void wait_empty(uint32_t bar) const { mbar_wait(bar, phase ^ 1u); }
+  // advance by `step` (0 or 1), without a branch on it: the tc32 consumers need more registers with `if (step)`
+  __device__ __forceinline__ void next(int slots, bool step = true) {
+    slot += step;
+    if (slot == slots) { slot = 0; phase ^= 1; }
+  }
+};
+
+// The filter tap of a K step and its (r, s).  K steps run chunk-major and tap-minor: within a channel chunk the tap
+// advances fastest, s before r.
+struct Tap {
+  int k = 0, r = 0, s = 0;
+  __device__ __forceinline__ void next(int kw) { ++k; if (++s == kw) { s = 0; ++r; } }
+};
+
 struct TileCoord {
   int prob, n_idx, img, ty, tx;
 };
@@ -369,6 +393,7 @@ inline void set_tiles(ConvTcParams& p, const vps_conv_args* a, int nprob, int tw
   p.block_n = block_n; p.n_tiles_n = vps::cdiv((a->cout + 15) / 16 * 16, block_n);
   p.kh = a->kh; p.kw = a->kw; p.sh = a->sh; p.sw = a->sw;
   p.cin_chunks = vps::cdiv(a->cin, kc);
+  p.nk_last = vps::cdiv(a->cin - (p.cin_chunks - 1) * kc, 16);
   p.nprob = nprob;
   p.tiles_per_prob = p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
   p.total_tiles = p.tiles_per_prob * nprob;

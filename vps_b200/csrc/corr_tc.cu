@@ -69,26 +69,25 @@ __device__ __forceinline__ void corr_consumer(const CorrParams& p, const CorrSme
   const bool leader = (threadIdx.x & 127) == 0;
   const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
   const int tiles_per_par = p.tiles_y * p.tiles_x;
-  int stage = 0; uint32_t phase = 0;
-  int bsel = 0; uint32_t bphase = 0;
+  RingPos ap, bp;       // f2 ring, f1 double buffer
   float d[NPIX / 2];
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const CorrTile t = corr_tile<R, S2>(p, tiles_per_par, tile);
-    mbar_wait(sm.bfull(bsel), bphase);
+    bp.wait_full(sm.bfull(bp.slot));
     for (int b = 0; b < NBLK; ++b) {
       for (int kc = 0; kc < p.kch; ++kc) {
-        mbar_wait(sm.afull(stage), phase);
+        ap.wait_full(sm.afull(ap.slot));
         // K-major, 128-byte rows (SWIZZLE_128B), 8-row groups 1 KiB apart
-        const uint64_t adesc = desc_at(desc_hi(128, 1024), sm.a_ring + stage * A_BYTES + (uint32_t)wg * 64u * 128u);
-        const uint64_t bdesc = desc_at(desc_hi(128, 1024), sm.b_buf + bsel * MAX_KCH * B_BYTES + kc * B_BYTES);
+        const uint64_t adesc = desc_at(desc_hi(128, 1024), sm.a_ring + ap.slot * A_BYTES + (uint32_t)wg * 64u * 128u);
+        const uint64_t bdesc = desc_at(desc_hi(128, 1024), sm.b_buf + bp.slot * MAX_KCH * B_BYTES + kc * B_BYTES);
         wg::fence();
 #pragma unroll
         for (int k = 0; k < KC / 16; ++k)
           wg::Mma<NPIX, F16>::run(d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)((kc | k) != 0));
         wg::commit();
         wg::wait<0>();
-        if (leader) mbar_arrive(sm.aempty(stage));
-        if (++stage == A_STAGES) { stage = 0; phase ^= 1; }
+        if (leader) mbar_arrive(sm.aempty(ap.slot));
+        ap.next(A_STAGES);
       }
       wg::fence_regs(d);
       // fragment element d[4q + 2h + e]: neighbourhood pixel n = 64 wg + 16 w + lane/4 + 8h, output pixel m = 8q + 2(lane%4) + e.
@@ -120,8 +119,8 @@ __device__ __forceinline__ void corr_consumer(const CorrParams& p, const CorrSme
         }
       }
     }
-    if (leader) mbar_arrive(sm.bempty(bsel));      // every MMA reading this f1 tile has completed
-    bsel ^= 1; if (bsel == 0) bphase ^= 1;
+    if (leader) mbar_arrive(sm.bempty(bp.slot));      // every MMA reading this f1 tile has completed
+    bp.next(2);
   }
 }
 
@@ -146,26 +145,25 @@ corr_tc_kernel(const __grid_constant__ CUtensorMap tmF1, const __grid_constant__
   const int tiles_per_par = p.tiles_y * p.tiles_x;
   if (warp == 0) {
     if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      int bsel = 0; uint32_t bphase = 0;
+      RingPos ap, bp;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         const CorrTile t = corr_tile<R, S2>(p, tiles_per_par, tile);
         // f1 tile (MMA B operand): resident for the whole tile, double-buffered across tiles
-        mbar_wait(sm.bempty(bsel), bphase ^ 1);
-        mbar_expect_tx(sm.bfull(bsel), b_tile_bytes);
+        bp.wait_empty(sm.bempty(bp.slot));
+        mbar_expect_tx(sm.bfull(bp.slot), b_tile_bytes);
         for (int kc = 0; kc < p.kch; ++kc)
-          tma_load_4d(sm.b_buf + bsel * MAX_KCH * B_BYTES + kc * B_BYTES, &tmF1, sm.bfull(bsel), kc * KC, t.x0 + t.px, t.y0 + t.py, t.img);
+          tma_load_4d(sm.b_buf + bp.slot * MAX_KCH * B_BYTES + kc * B_BYTES, &tmF1, sm.bfull(bp.slot), kc * KC, t.x0 + t.px, t.y0 + t.py, t.img);
         // f2 neighbourhood blocks (MMA A operand): 4 rows x 32 columns of same-parity pixels each
         for (int b = 0; b < NBLK; ++b) {
           for (int kc = 0; kc < p.kch; ++kc) {
-            mbar_wait(sm.aempty(stage), phase ^ 1);
-            mbar_expect_tx(sm.afull(stage), A_BYTES);
-            tma_load_4d(sm.a_ring + stage * A_BYTES, &tmF2, sm.afull(stage), kc * KC, t.x0 + t.px - R * S2,
+            ap.wait_empty(sm.aempty(ap.slot));
+            mbar_expect_tx(sm.afull(ap.slot), A_BYTES);
+            tma_load_4d(sm.a_ring + ap.slot * A_BYTES, &tmF2, sm.afull(ap.slot), kc * KC, t.x0 + t.px - R * S2,
                         t.y0 + t.py + (4 * b - R) * S2, t.img);
-            if (++stage == A_STAGES) { stage = 0; phase ^= 1; }
+            ap.next(A_STAGES);
           }
         }
-        bsel ^= 1; if (bsel == 0) bphase ^= 1;
+        bp.next(2);
       }
     }
   } else if (warp >= 4) {
