@@ -7,6 +7,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <type_traits>
+
 #include "../../include/vps_b200.h"
 
 namespace vps {
@@ -43,6 +45,26 @@ bool encode_nhwc(CUtensorMap* m, const vps_tensor& t, CUtensorMapDataType type, 
 
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
+// blocks of a grid-stride launch over `total` items, capped at 148 * 32: 32 blocks per SM of the 148-SM B200 (an H100 has
+// 132 SMs; the cap has not been retuned for it)
+static inline int grid_for(int64_t total, int threads = 256) {
+  int64_t b = (total + threads - 1) / threads;
+  const int64_t cap = 148 * 32;
+  return (int)(b > cap ? cap : (b < 1 ? 1 : b));
+}
+
+#define VPS_GRID_STRIDE(i, total) \
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < (total); i += (int64_t)gridDim.x * blockDim.x)
+
+// decompose flat index over [n,h,w,c] with c fastest
+#define VPS_DECOMP_NHWC(i, T_, n_, y_, x_, c_)  \
+  const int c_ = (int)((i) % (T_).c);           \
+  int64_t t__ = (i) / (T_).c;                   \
+  const int x_ = (int)(t__ % (T_).w);           \
+  t__ /= (T_).w;                                \
+  const int y_ = (int)(t__ % (T_).h);           \
+  const int n_ = (int)(t__ / (T_).h)
+
 // ---- typed element access (activations are f32 or bf16) ----
 template <typename T>
 __device__ __forceinline__ float ldf(const T* p);
@@ -78,7 +100,7 @@ static inline TV<T> tv(const vps_tensor& t) {
   return v;
 }
 
-// dispatch on (in dtype, out dtype) pairs used by the memory-bound kernels
+// binds T to the element type of `dtype` (f32 or bf16); nest it to bind a second type (input / output, data / flow)
 #define VPS_DISPATCH_T(dtype, T, ...)                         \
   do {                                                        \
     if ((dtype) == VPS_F32) { using T = float; __VA_ARGS__; } \
@@ -135,7 +157,8 @@ __device__ __forceinline__ void stv(T* p, const float (&v)[V]) {
 }
 // can tensor t be accessed with V-wide vectors of its dtype over its first `c` channels?
 static inline bool vec_ok(const vps_tensor& t, int c) {
-  const int V = t.dtype == VPS_F32 ? 4 : 8;
+  int V;
+  VPS_DISPATCH_T(t.dtype, T, V = VecW<T>::value);
   return c % V == 0 && t.cs % V == 0 && ((uintptr_t)t.ptr & 15) == 0;
 }
 // launch geometry of the (x*chunks, y, n) pixel grid
@@ -159,3 +182,16 @@ __device__ __forceinline__ float vps_bilerp(float v00, float v01, float v10, flo
   const int t__ = blockIdx.x * blockDim.x + threadIdx.x;                 \
   if (t__ >= (OUT).w * chunks__) return;                                 \
   const int c_ = (t__ % chunks__) * (V), x_ = t__ / chunks__, y_ = blockIdx.y, n_ = blockIdx.z
+
+// channel width V of a VPS_PIX_COORDS launch, bound at compile time: VW if `vec` (every tensor passed vps::vec_ok), else 1
+#define VPS_WITH_V(VW, vec, V, ...)                     \
+  do {                                                  \
+    if (vec) { constexpr int V = VW; __VA_ARGS__; }     \
+    else { constexpr int V = 1; __VA_ARGS__; }          \
+  } while (0)
+// binds T from `dtype` and V = VecW<T>::value if `vec`, else 1; the launch covers vps::pix_grid(w, c / V, h, n)
+#define VPS_DISPATCH_V(dtype, vec, T, V, ...) VPS_DISPATCH_T(dtype, T, VPS_WITH_V(vps::VecW<T>::value, vec, V, __VA_ARGS__))
+// input / output pair: the vector arm exists only where TI == TO (a mixed pair has no vector instances, V = 1)
+#define VPS_DISPATCH_IN_OUT_V(in_dtype, out_dtype, vec, TI, TO, V, ...)                  \
+  VPS_DISPATCH_T(in_dtype, TI, VPS_DISPATCH_T(out_dtype, TO,                             \
+    VPS_WITH_V((std::is_same<TI, TO>::value ? vps::VecW<TI>::value : 1), vec, V, __VA_ARGS__)))

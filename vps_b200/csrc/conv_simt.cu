@@ -128,16 +128,6 @@ __global__ void pack_weights_simt_kernel(const float* __restrict__ src, const fl
   }
 }
 
-template <typename TI, typename TO>
-int launch_simt(const vps_conv_args* a, const ConvSimtParams& p, dim3 grid, cudaStream_t st) {
-  if (a->res.ptr && a->res.dtype == VPS_BF16)
-    conv_simt_kernel<TI, TO, __nv_bfloat16><<<grid, 256, 0, st>>>(p);
-  else
-    conv_simt_kernel<TI, TO, float><<<grid, 256, 0, st>>>(p);
-  VPS_CUDA_LAST("conv_simt_kernel");
-  return VPS_OK;
-}
-
 }  // namespace
 
 extern "C" int vps_pack_weights_simt(const float* w, const float* scale, float* dst, int cout, int cin, int kh,
@@ -164,9 +154,9 @@ extern "C" int vps_conv2d_simt(const vps_conv_args* a, void* stream) {
   p.total_pix = (int64_t)a->x.n * a->oh * a->ow;
   if (p.total_pix == 0) return VPS_OK;
   dim3 grid((unsigned)((p.total_pix + TP - 1) / TP), (unsigned)((a->cout + TC - 1) / TC));
-  cudaStream_t st = (cudaStream_t)stream;
-  if (a->x.dtype == VPS_F32 && a->y.dtype == VPS_F32) return launch_simt<float, float>(a, p, grid, st);
-  if (a->x.dtype == VPS_BF16 && a->y.dtype == VPS_BF16) return launch_simt<__nv_bfloat16, __nv_bfloat16>(a, p, grid, st);
-  if (a->x.dtype == VPS_BF16 && a->y.dtype == VPS_F32) return launch_simt<__nv_bfloat16, float>(a, p, grid, st);
-  return launch_simt<float, __nv_bfloat16>(a, p, grid, st);
+  // without a residual the kernel never reads one: the fp32-residual instance runs
+  VPS_DISPATCH_T(a->x.dtype, TI, VPS_DISPATCH_T(a->y.dtype, TO, VPS_DISPATCH_T(a->res.ptr ? a->res.dtype : VPS_F32, TR,
+      (conv_simt_kernel<TI, TO, TR><<<grid, 256, 0, (cudaStream_t)stream>>>(p)))));
+  VPS_CUDA_LAST("conv_simt_kernel");
+  return VPS_OK;
 }

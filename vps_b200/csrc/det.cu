@@ -7,14 +7,6 @@
 
 namespace {
 
-inline int grid_for(int64_t total, int threads = 256) {
-  int64_t b = (total + threads - 1) / threads;
-  const int64_t cap = 148 * 32;
-  return (int)(b > cap ? cap : (b < 1 ? 1 : b));
-}
-#define GRID_STRIDE(i, total) \
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < (total); i += (int64_t)gridDim.x * blockDim.x)
-
 // ------------------------------------------------------------------ RoIAlign
 constexpr int MAXLEV = 4;
 template <typename T>
@@ -222,7 +214,7 @@ __global__ void gather_rows_kernel(const float* __restrict__ src, const int32_t*
                                    const int* __restrict__ n_dev, int width, float* __restrict__ dst) {
   const int n = n_dev ? min(*n_dev, n_cap) : n_cap;
   const int64_t total = (int64_t)n_cap * width;
-  GRID_STRIDE(i, total) {
+  VPS_GRID_STRIDE(i, total) {
     const int r = (int)(i / width), c = (int)(i % width);
     dst[i] = r < n ? src[(int64_t)idx[r] * width + c] : 0.f;
   }
@@ -447,7 +439,7 @@ __global__ void select_class_kernel(vps::TV<const T> logits, const int32_t* __re
                                     float* __restrict__ out) {
   const int64_t per = (int64_t)logits.h * logits.w;
   const int64_t total = (int64_t)k * per;
-  GRID_STRIDE(i, total) {
+  VPS_GRID_STRIDE(i, total) {
     const int r = (int)(i / per);
     const int64_t pix = i % per;
     out[i] = vps::ldf<T>(logits.p + ((int64_t)r * per + pix) * logits.cs + cls_idx[r]);
@@ -491,19 +483,14 @@ extern "C" int vps_roi_align(const vps_tensor* feats, const int* strides, int nl
     VPS_CHECK_ARG(feats[i].dtype == out->dtype && feats[i].c >= out->c, "roi_align: level %d dtype/channels", i);
     vec = vec && vps::vec_ok(feats[i], out->c);
   }
-  cudaStream_t st = (cudaStream_t)stream;
-#define RA_LAUNCH(T, V)                                                                                     \
-  do {                                                                                                      \
-    Feats<T> fs;                                                                                            \
-    fs.n = nlev;                                                                                            \
-    for (int i = 0; i < nlev; ++i) { fs.l[i] = vps::tv<const T>(feats[i]); fs.scale[i] = 1.0f / (float)strides[i]; } \
-    for (int i = nlev; i < MAXLEV; ++i) { fs.l[i] = fs.l[nlev - 1]; fs.scale[i] = fs.scale[nlev - 1]; }       \
-    roi_align_kernel<T, V><<<vps::pix_grid(out->w, out->c / V, out->h, nroi, 128), 128, 0, st>>>(           \
-        fs, rois, nroi, nroi_dev, vps::tv<T>(*out), out->h, sample_num);                                    \
-  } while (0)
-  if (out->dtype == VPS_F32) { if (vec) RA_LAUNCH(float, 4); else RA_LAUNCH(float, 1); }
-  else { if (vec) RA_LAUNCH(__nv_bfloat16, 8); else RA_LAUNCH(__nv_bfloat16, 1); }
-#undef RA_LAUNCH
+  VPS_DISPATCH_V(out->dtype, vec, T, V, {
+    Feats<T> fs;
+    fs.n = nlev;
+    for (int i = 0; i < nlev; ++i) { fs.l[i] = vps::tv<const T>(feats[i]); fs.scale[i] = 1.0f / (float)strides[i]; }
+    for (int i = nlev; i < MAXLEV; ++i) { fs.l[i] = fs.l[nlev - 1]; fs.scale[i] = fs.scale[nlev - 1]; }
+    roi_align_kernel<T, V><<<vps::pix_grid(out->w, out->c / V, out->h, nroi, 128), 128, 0, (cudaStream_t)stream>>>(
+        fs, rois, nroi, nroi_dev, vps::tv<T>(*out), out->h, sample_num);
+  });
   VPS_CUDA_LAST("roi_align");
   return VPS_OK;
 }
@@ -570,7 +557,7 @@ extern "C" int vps_nms(const float* dets, int n, const int* n_dev, float thr, in
 extern "C" int vps_gather_rows(const float* src, const int32_t* idx, int n, const int* n_dev, int width, float* dst,
                                void* stream) {
   if (n <= 0) return VPS_OK;
-  gather_rows_kernel<<<grid_for((int64_t)n * width), 256, 0, (cudaStream_t)stream>>>(src, idx, n, n_dev, width, dst);
+  gather_rows_kernel<<<vps::grid_for((int64_t)n * width), 256, 0, (cudaStream_t)stream>>>(src, idx, n, n_dev, width, dst);
   VPS_CUDA_LAST("gather_rows");
   return VPS_OK;
 }
@@ -602,7 +589,7 @@ extern "C" int vps_track_assign(const float* emb, const float* ref_emb, int k, i
   float* match_like = dots + (int64_t)k * m;
   float* best_scores = match_like + k;
   int32_t* best_ids = (int32_t*)(best_scores + cap);
-  track_dot_kernel<<<grid_for((int64_t)k * m * 32), 256, 0, st>>>(emb, ref_emb, k, m, dim, dots);
+  track_dot_kernel<<<vps::grid_for((int64_t)k * m * 32), 256, 0, st>>>(emb, ref_emb, k, m, dim, dots);
   VPS_CUDA_LAST("track_dot");
   track_score_kernel<<<vps::cdiv((int64_t)k * 32, 128), 128, 0, st>>>(dots, k, m, det_boxes, ref_boxes, det_labels,
                                                                      ref_labels, cls_prob, c0, c1, c2, comp_scores,
@@ -640,7 +627,7 @@ extern "C" int vps_select_class(const vps_tensor* logits, const int32_t* cls_idx
   if (k <= 0) return VPS_OK;
   VPS_CHECK_ARG(logits->n >= k, "select_class: k");
   const int64_t total = (int64_t)k * logits->h * logits->w;
-  VPS_DISPATCH_T(logits->dtype, T, (select_class_kernel<T><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(
+  VPS_DISPATCH_T(logits->dtype, T, (select_class_kernel<T><<<vps::grid_for(total), 256, 0, (cudaStream_t)stream>>>(
                                        vps::tv<const T>(*logits), cls_idx, k, out)));
   VPS_CUDA_LAST("select_class");
   return VPS_OK;

@@ -155,12 +155,6 @@ __global__ void channelnorm_kernel(vps::TV<const T> a, vps::TV<const T> b, int h
   }
 }
 
-inline int grid_for(int64_t total, int threads) {
-  int64_t b = (total + threads - 1) / threads;
-  const int64_t cap = 148 * 32;
-  return (int)(b > cap ? cap : (b < 1 ? 1 : b));
-}
-
 }  // namespace
 
 extern "C" int vps_correlation_tc(const vps_tensor* f1, const vps_tensor* f2, const vps_tensor* out, int pad, int max_disp,
@@ -202,19 +196,10 @@ extern "C" int vps_resample2d(const vps_tensor* src, const vps_tensor* flow, con
   VPS_CHECK_ARG(src->dtype == out->dtype && src->c == out->c && flow->c >= 2, "resample2d: bad args");
   VPS_CHECK_ARG(flow->h == out->h && flow->w == out->w, "resample2d: flow/out size");
   if (!((int64_t)out->n * out->h * out->w * out->c)) return VPS_OK;
-  cudaStream_t st = (cudaStream_t)stream;
   const bool vec = vps::vec_ok(*src, out->c) && vps::vec_ok(*out, out->c);
-#define RS_LAUNCH(T, TF, V)                                                                               \
-  resample2d_kernel<T, TF, V><<<vps::pix_grid(out->w, out->c / V, out->h, out->n), 256, 0, st>>>(          \
-      vps::tv<const T>(*src), vps::tv<const TF>(*flow), vps::tv<T>(*out))
-  if (out->dtype == VPS_F32) {
-    if (flow->dtype == VPS_F32) { if (vec) RS_LAUNCH(float, float, 4); else RS_LAUNCH(float, float, 1); }
-    else { if (vec) RS_LAUNCH(float, __nv_bfloat16, 4); else RS_LAUNCH(float, __nv_bfloat16, 1); }
-  } else {
-    if (flow->dtype == VPS_F32) { if (vec) RS_LAUNCH(__nv_bfloat16, float, 8); else RS_LAUNCH(__nv_bfloat16, float, 1); }
-    else { if (vec) RS_LAUNCH(__nv_bfloat16, __nv_bfloat16, 8); else RS_LAUNCH(__nv_bfloat16, __nv_bfloat16, 1); }
-  }
-#undef RS_LAUNCH
+  VPS_DISPATCH_T(flow->dtype, TF, VPS_DISPATCH_V(out->dtype, vec, T, V,
+      (resample2d_kernel<T, TF, V><<<vps::pix_grid(out->w, out->c / V, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(
+          vps::tv<const T>(*src), vps::tv<const TF>(*flow), vps::tv<T>(*out)))));
   VPS_CUDA_LAST("resample2d_kernel");
   return VPS_OK;
 }
@@ -224,17 +209,10 @@ extern "C" int vps_channelnorm(const vps_tensor* a, const vps_tensor* b, const v
   if (b) VPS_CHECK_ARG(b->dtype == a->dtype && b->c == a->c && b->h == a->h && b->w == a->w, "channelnorm: b");
   const int64_t total = (int64_t)a->n * a->h * a->w;
   if (!total) return VPS_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int g = grid_for(total, 256);
   vps_tensor bb = b ? *b : *a;
-  VPS_DISPATCH_T(a->dtype, T, {
-    if (out->dtype == VPS_F32)
-      channelnorm_kernel<T, float><<<g, 256, 0, st>>>(vps::tv<const T>(*a), vps::tv<const T>(bb), b != nullptr,
-                                                     vps::tv<float>(*out), total);
-    else
-      channelnorm_kernel<T, __nv_bfloat16><<<g, 256, 0, st>>>(vps::tv<const T>(*a), vps::tv<const T>(bb),
-                                                             b != nullptr, vps::tv<__nv_bfloat16>(*out), total);
-  });
+  VPS_DISPATCH_T(a->dtype, T, VPS_DISPATCH_T(out->dtype, TO,
+      (channelnorm_kernel<T, TO><<<vps::grid_for(total), 256, 0, (cudaStream_t)stream>>>(
+          vps::tv<const T>(*a), vps::tv<const T>(bb), b != nullptr, vps::tv<TO>(*out), total))));
   VPS_CUDA_LAST("channelnorm_kernel");
   return VPS_OK;
 }
@@ -292,7 +270,7 @@ extern "C" int vps_flownet_input(const float* img_nchw, const float* ref_nchw, i
   dim3 g1(148, 3);
   flownet_sums_kernel<<<g1, 256, 0, st>>>(img_nchw, ref_nchw, hw, s, m, sums_ws);
   VPS_CUDA_LAST("flownet_sums");
-  VPS_DISPATCH_T(x->dtype, T, (flownet_input_kernel<T><<<grid_for(hw * 6, 256), 256, 0, st>>>(img_nchw, ref_nchw, hw, s, m,
+  VPS_DISPATCH_T(x->dtype, T, (flownet_input_kernel<T><<<vps::grid_for(hw * 6), 256, 0, st>>>(img_nchw, ref_nchw, hw, s, m,
                                                                                             sums_ws, rgb_max, vps::tv<T>(*x))));
   VPS_CUDA_LAST("flownet_input");
   return VPS_OK;
@@ -341,11 +319,8 @@ extern "C" int vps_flow_deconv(const vps_tensor* x, const float* w_iohw_host, co
   W.b[0] = bias_host ? bias_host[0] : 0.f;
   W.b[1] = bias_host ? bias_host[1] : 0.f;
   dim3 grid(vps::cdiv(y->w, 128), y->h, y->n);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (x->dtype == VPS_F32 && y->dtype == VPS_F32) flow_deconv_kernel<float, float><<<grid, 128, 0, st>>>(vps::tv<const float>(*x), vps::tv<float>(*y), W);
-  else if (x->dtype == VPS_F32) flow_deconv_kernel<float, __nv_bfloat16><<<grid, 128, 0, st>>>(vps::tv<const float>(*x), vps::tv<__nv_bfloat16>(*y), W);
-  else if (y->dtype == VPS_F32) flow_deconv_kernel<__nv_bfloat16, float><<<grid, 128, 0, st>>>(vps::tv<const __nv_bfloat16>(*x), vps::tv<float>(*y), W);
-  else flow_deconv_kernel<__nv_bfloat16, __nv_bfloat16><<<grid, 128, 0, st>>>(vps::tv<const __nv_bfloat16>(*x), vps::tv<__nv_bfloat16>(*y), W);
+  VPS_DISPATCH_T(x->dtype, TI, VPS_DISPATCH_T(y->dtype, TO,
+      (flow_deconv_kernel<TI, TO><<<grid, 128, 0, (cudaStream_t)stream>>>(vps::tv<const TI>(*x), vps::tv<TO>(*y), W))));
   VPS_CUDA_LAST("flow_deconv");
   return VPS_OK;
 }
@@ -495,12 +470,9 @@ extern "C" int vps_flownet_stage(const vps_tensor* x6, const vps_tensor* flow_lo
                     cat->h == x6->h && cat->w == x6->w && cat->n == x6->n && flow_lo->n == x6->n, "flownet_stage: shapes");
   if (!((int64_t)cat->n * cat->h * cat->w)) return VPS_OK;
   dim3 grid((unsigned)vps::cdiv(cat->w, 256), (unsigned)cat->h, (unsigned)cat->n);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (cat->dtype == VPS_F32)
-    flownet_stage_kernel<float><<<grid, 256, 0, st>>>(vps::tv<const float>(*x6), vps::tv<const float>(*flow_lo), mul, inv, vps::tv<float>(*cat), cat_pad(cat));
-  else
-    flownet_stage_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(vps::tv<const __nv_bfloat16>(*x6), vps::tv<const float>(*flow_lo), mul, inv,
-                                                             vps::tv<__nv_bfloat16>(*cat), cat_pad(cat));
+  VPS_DISPATCH_T(cat->dtype, T,
+                 (flownet_stage_kernel<T><<<grid, 256, 0, (cudaStream_t)stream>>>(vps::tv<const T>(*x6), vps::tv<const float>(*flow_lo), mul,
+                                                                                 inv, vps::tv<T>(*cat), cat_pad(cat))));
   VPS_CUDA_LAST("flownet_stage");
   return VPS_OK;
 }
@@ -511,14 +483,10 @@ extern "C" int vps_flownet_cat3(const vps_tensor* x6, const vps_tensor* s2_flow_
                     cat->c == 11 && cat->dtype == x6->dtype && cat->h == x6->h && cat->w == x6->w && cat->n == x6->n, "flownet_cat3: shapes");
   if (!((int64_t)cat->n * cat->h * cat->w)) return VPS_OK;
   dim3 grid((unsigned)vps::cdiv(cat->w, 256), (unsigned)cat->h, (unsigned)cat->n);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (cat->dtype == VPS_F32)
-    flownet_cat3_kernel<float><<<grid, 256, 0, st>>>(vps::tv<const float>(*x6), vps::tv<const float>(*s2_flow_lo), vps::tv<const float>(*sd_flow_lo),
-                                                     mul_s2, mul_sd, vps::tv<float>(*cat), cat_pad(cat));
-  else
-    flownet_cat3_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(vps::tv<const __nv_bfloat16>(*x6), vps::tv<const float>(*s2_flow_lo),
-                                                            vps::tv<const float>(*sd_flow_lo), mul_s2, mul_sd, vps::tv<__nv_bfloat16>(*cat),
-                                                            cat_pad(cat));
+  VPS_DISPATCH_T(cat->dtype, T,
+                 (flownet_cat3_kernel<T><<<grid, 256, 0, (cudaStream_t)stream>>>(vps::tv<const T>(*x6), vps::tv<const float>(*s2_flow_lo),
+                                                                                vps::tv<const float>(*sd_flow_lo), mul_s2, mul_sd,
+                                                                                vps::tv<T>(*cat), cat_pad(cat))));
   VPS_CUDA_LAST("flownet_cat3");
   return VPS_OK;
 }

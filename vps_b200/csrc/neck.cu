@@ -4,21 +4,6 @@
 
 namespace {
 
-inline int grid_for(int64_t total, int threads = 256) {
-  int64_t b = (total + threads - 1) / threads;
-  const int64_t cap = 148 * 32;
-  return (int)(b > cap ? cap : (b < 1 ? 1 : b));
-}
-#define GRID_STRIDE(i, total) \
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < (total); i += (int64_t)gridDim.x * blockDim.x)
-#define DECOMP_NHWC(i, T_, n_, y_, x_, c_)      \
-  const int c_ = (int)((i) % (T_).c);           \
-  int64_t t__ = (i) / (T_).c;                   \
-  const int x_ = (int)(t__ % (T_).w);           \
-  t__ /= (T_).w;                                \
-  const int y_ = (int)(t__ % (T_).h);           \
-  const int n_ = (int)(t__ / (T_).h)
-
 constexpr int MAXLEV = 8;
 template <typename T>
 struct Levels {
@@ -162,7 +147,7 @@ __global__ void tcea_combine_kernel(vps::TV<const T> fea, vps::TV<const T> att, 
 template <typename T, typename TOF>
 __global__ void deform_im2col_kernel(vps::TV<const T> x, vps::TV<const TOF> off, vps::TV<T> cols, int64_t total) {
   const int C = x.c, H = x.h, W = x.w;
-  GRID_STRIDE(i, total) {
+  VPS_GRID_STRIDE(i, total) {
     const int c = (int)(i % C);
     int64_t t = i / C;
     const int k = (int)(t % 9); t /= 9;
@@ -243,20 +228,6 @@ __global__ void deform_im2col_bf16x8_kernel(vps::TV<const __nv_bfloat16> x, vps:
 
 }  // namespace
 
-#define LAUNCH_V(T_dtype, vec, KERN, w, c, h, n, ...)                                                   \
-  do {                                                                                                  \
-    cudaStream_t st__ = (cudaStream_t)stream;                                                           \
-    if ((T_dtype) == VPS_F32) {                                                                         \
-      using T = float;                                                                                  \
-      if (vec) KERN<T, 4><<<vps::pix_grid(w, (c) / 4, h, n), 256, 0, st__>>>(__VA_ARGS__);             \
-      else KERN<T, 1><<<vps::pix_grid(w, c, h, n), 256, 0, st__>>>(__VA_ARGS__);                       \
-    } else {                                                                                            \
-      using T = __nv_bfloat16;                                                                          \
-      if (vec) KERN<T, 8><<<vps::pix_grid(w, (c) / 8, h, n), 256, 0, st__>>>(__VA_ARGS__);             \
-      else KERN<T, 1><<<vps::pix_grid(w, c, h, n), 256, 0, st__>>>(__VA_ARGS__);                       \
-    }                                                                                                   \
-  } while (0)
-
 extern "C" int vps_bfp_gather(const vps_tensor* levels, int nlev, const vps_tensor* out, void* stream) {
   VPS_CHECK_ARG(nlev >= 1 && nlev <= MAXLEV, "bfp_gather: nlev");
   if (!((int64_t)out->n * out->h * out->w * out->c)) return VPS_OK;
@@ -265,17 +236,11 @@ extern "C" int vps_bfp_gather(const vps_tensor* levels, int nlev, const vps_tens
     VPS_CHECK_ARG(levels[i].dtype == out->dtype && levels[i].c >= out->c, "bfp_gather: level %d", i);
     vec = vec && vps::vec_ok(levels[i], out->c);
   }
-  if (out->dtype == VPS_F32) {
-    Levels<float> lv; lv.n = nlev;
-    for (int i = 0; i < nlev; ++i) lv.l[i] = vps::tv<const float>(levels[i]);
-    if (vec) bfp_gather_kernel<float, 4><<<vps::pix_grid(out->w, out->c / 4, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(lv, vps::tv<float>(*out));
-    else bfp_gather_kernel<float, 1><<<vps::pix_grid(out->w, out->c, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(lv, vps::tv<float>(*out));
-  } else {
-    Levels<__nv_bfloat16> lv; lv.n = nlev;
-    for (int i = 0; i < nlev; ++i) lv.l[i] = vps::tv<const __nv_bfloat16>(levels[i]);
-    if (vec) bfp_gather_kernel<__nv_bfloat16, 8><<<vps::pix_grid(out->w, out->c / 8, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(lv, vps::tv<__nv_bfloat16>(*out));
-    else bfp_gather_kernel<__nv_bfloat16, 1><<<vps::pix_grid(out->w, out->c, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(lv, vps::tv<__nv_bfloat16>(*out));
-  }
+  VPS_DISPATCH_V(out->dtype, vec, T, V, {
+    Levels<T> lv; lv.n = nlev;
+    for (int i = 0; i < nlev; ++i) lv.l[i] = vps::tv<const T>(levels[i]);
+    bfp_gather_kernel<T, V><<<vps::pix_grid(out->w, out->c / V, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(lv, vps::tv<T>(*out));
+  });
   VPS_CUDA_LAST("bfp_gather");
   return VPS_OK;
 }
@@ -284,8 +249,9 @@ extern "C" int vps_bfp_scatter(const vps_tensor* bsf, const vps_tensor* in, cons
   VPS_CHECK_ARG(in->h == out->h && in->w == out->w && bsf->dtype == out->dtype && in->dtype == out->dtype, "bfp_scatter: args");
   if (!((int64_t)out->n * out->h * out->w * out->c)) return VPS_OK;
   const bool vec = vps::vec_ok(*bsf, out->c) && vps::vec_ok(*in, out->c) && vps::vec_ok(*out, out->c);
-  LAUNCH_V(out->dtype, vec, bfp_scatter_kernel, out->w, out->c, out->h, out->n, vps::tv<const T>(*bsf), vps::tv<const T>(*in),
-           vps::tv<T>(*out));
+  VPS_DISPATCH_V(out->dtype, vec, T, V,
+                 (bfp_scatter_kernel<T, V><<<vps::pix_grid(out->w, out->c / V, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(
+                     vps::tv<const T>(*bsf), vps::tv<const T>(*in), vps::tv<T>(*out))));
   VPS_CUDA_LAST("bfp_scatter");
   return VPS_OK;
 }
@@ -295,18 +261,9 @@ extern "C" int vps_flow_warp(const vps_tensor* src, const vps_tensor* flow, cons
                 "flow_warp: args");
   if (!((int64_t)out->n * out->h * out->w * out->c)) return VPS_OK;
   const bool vec = vps::vec_ok(*src, out->c) && vps::vec_ok(*out, out->c);
-  cudaStream_t st = (cudaStream_t)stream;
-#define FW_LAUNCH(T, TF, V)                                                                                         \
-  flow_warp_kernel<T, TF, V><<<vps::pix_grid(out->w, out->c / V, out->h, out->n), 256, 0, st>>>(                    \
-      vps::tv<const T>(*src), vps::tv<const TF>(*flow), vps::tv<T>(*out))
-  if (out->dtype == VPS_F32) {
-    if (flow->dtype == VPS_F32) { if (vec) FW_LAUNCH(float, float, 4); else FW_LAUNCH(float, float, 1); }
-    else { if (vec) FW_LAUNCH(float, __nv_bfloat16, 4); else FW_LAUNCH(float, __nv_bfloat16, 1); }
-  } else {
-    if (flow->dtype == VPS_F32) { if (vec) FW_LAUNCH(__nv_bfloat16, float, 8); else FW_LAUNCH(__nv_bfloat16, float, 1); }
-    else { if (vec) FW_LAUNCH(__nv_bfloat16, __nv_bfloat16, 8); else FW_LAUNCH(__nv_bfloat16, __nv_bfloat16, 1); }
-  }
-#undef FW_LAUNCH
+  VPS_DISPATCH_T(flow->dtype, TF, VPS_DISPATCH_V(out->dtype, vec, T, V,
+      (flow_warp_kernel<T, TF, V><<<vps::pix_grid(out->w, out->c / V, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(
+          vps::tv<const T>(*src), vps::tv<const TF>(*flow), vps::tv<T>(*out)))));
   VPS_CUDA_LAST("flow_warp");
   return VPS_OK;
 }
@@ -319,15 +276,12 @@ extern "C" int vps_tcea_temporal(const vps_tensor* fea0, const vps_tensor* fea1,
   const int64_t npix = (int64_t)out->n * out->h * out->w;
   if (!npix) return VPS_OK;
   const int C = fea0->c;
-  const int Vw = out->dtype == VPS_F32 ? 4 : 8;
-  const bool vec = C % Vw == 0 && vps::vec_ok(*fea0, C) && vps::vec_ok(*fea1, C) && vps::vec_ok(*emb0, C) && vps::vec_ok(*emb1, C) &&
+  const bool vec = vps::vec_ok(*fea0, C) && vps::vec_ok(*fea1, C) && vps::vec_ok(*emb0, C) && vps::vec_ok(*emb1, C) &&
                    vps::vec_ok(*emb_ref, C) && vps::vec_ok(*out, 2 * C);
-#define TT_LAUNCH(T, V) tcea_temporal_kernel<T, V><<<grid_for(npix * 32), 256, 0, (cudaStream_t)stream>>>(                \
-      vps::tv<const T>(*fea0), vps::tv<const T>(*fea1), vps::tv<const T>(*emb0), vps::tv<const T>(*emb1), vps::tv<const T>(*emb_ref), \
-      vps::tv<T>(*out), npix)
-  if (out->dtype == VPS_F32) { if (vec) TT_LAUNCH(float, 4); else TT_LAUNCH(float, 1); }
-  else { if (vec) TT_LAUNCH(__nv_bfloat16, 8); else TT_LAUNCH(__nv_bfloat16, 1); }
-#undef TT_LAUNCH
+  VPS_DISPATCH_V(out->dtype, vec, T, V,
+                 (tcea_temporal_kernel<T, V><<<vps::grid_for(npix * 32), 256, 0, (cudaStream_t)stream>>>(
+                     vps::tv<const T>(*fea0), vps::tv<const T>(*fea1), vps::tv<const T>(*emb0), vps::tv<const T>(*emb1),
+                     vps::tv<const T>(*emb_ref), vps::tv<T>(*out), npix)));
   VPS_CUDA_LAST("tcea_temporal");
   return VPS_OK;
 }
@@ -337,8 +291,9 @@ extern "C" int vps_tcea_combine(const vps_tensor* fea, const vps_tensor* att, co
   VPS_CHECK_ARG(fea->dtype == out->dtype && att->dtype == out->dtype && att_add->dtype == out->dtype, "tcea_combine: dtype");
   if (!((int64_t)out->n * out->h * out->w * out->c)) return VPS_OK;
   const bool vec = vps::vec_ok(*fea, out->c) && vps::vec_ok(*att, out->c) && vps::vec_ok(*att_add, out->c) && vps::vec_ok(*out, out->c);
-  LAUNCH_V(out->dtype, vec, tcea_combine_kernel, out->w, out->c, out->h, out->n, vps::tv<const T>(*fea), vps::tv<const T>(*att),
-           vps::tv<const T>(*att_add), vps::tv<T>(*out));
+  VPS_DISPATCH_V(out->dtype, vec, T, V,
+                 (tcea_combine_kernel<T, V><<<vps::pix_grid(out->w, out->c / V, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(
+                     vps::tv<const T>(*fea), vps::tv<const T>(*att), vps::tv<const T>(*att_add), vps::tv<T>(*out))));
   VPS_CUDA_LAST("tcea_combine");
   return VPS_OK;
 }
@@ -354,23 +309,15 @@ extern "C" int vps_deform_im2col(const vps_tensor* x, const vps_tensor* offset, 
     VPS_CHECK_ARG(tot8 < (1ll << 31) - (148ll * 64 * 256), "deform_im2col: tensor too large for 32-bit indexing");
     int64_t blocks = (tot8 + 255) / 256;
     if (blocks > 148 * 64) blocks = 148 * 64;
-    if (offset->dtype == VPS_F32)
-      deform_im2col_bf16x8_kernel<float><<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(
-          vps::tv<const __nv_bfloat16>(*x), vps::tv<const float>(*offset), vps::tv<__nv_bfloat16>(*cols), tot8);
-    else
-      deform_im2col_bf16x8_kernel<__nv_bfloat16><<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(
-          vps::tv<const __nv_bfloat16>(*x), vps::tv<const __nv_bfloat16>(*offset), vps::tv<__nv_bfloat16>(*cols), tot8);
+    VPS_DISPATCH_T(offset->dtype, TOF,
+                   (deform_im2col_bf16x8_kernel<TOF><<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(
+                       vps::tv<const __nv_bfloat16>(*x), vps::tv<const TOF>(*offset), vps::tv<__nv_bfloat16>(*cols), tot8)));
     VPS_CUDA_LAST("deform_im2col_bf16x8");
     return VPS_OK;
   }
-  VPS_DISPATCH_T(x->dtype, T, {
-    if (offset->dtype == VPS_F32)
-      deform_im2col_kernel<T, float><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(
-          vps::tv<const T>(*x), vps::tv<const float>(*offset), vps::tv<T>(*cols), total);
-    else
-      deform_im2col_kernel<T, __nv_bfloat16><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(
-          vps::tv<const T>(*x), vps::tv<const __nv_bfloat16>(*offset), vps::tv<T>(*cols), total);
-  });
+  VPS_DISPATCH_T(x->dtype, T, VPS_DISPATCH_T(offset->dtype, TOF,
+      (deform_im2col_kernel<T, TOF><<<vps::grid_for(total), 256, 0, (cudaStream_t)stream>>>(
+          vps::tv<const T>(*x), vps::tv<const TOF>(*offset), vps::tv<T>(*cols), total))));
   VPS_CUDA_LAST("deform_im2col");
   return VPS_OK;
 }

@@ -6,34 +6,16 @@
 
 namespace {
 
-inline int grid_for(int64_t total, int threads = 256) {
-  int64_t b = (total + threads - 1) / threads;
-  const int64_t cap = 148 * 32;
-  return (int)(b > cap ? cap : (b < 1 ? 1 : b));
-}
-
-#define GRID_STRIDE(i, total) \
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < (total); i += (int64_t)gridDim.x * blockDim.x)
-
-// decompose flat index over [n,h,w,c] with c fastest
-#define DECOMP_NHWC(i, T_, n_, y_, x_, c_)      \
-  const int c_ = (int)((i) % (T_).c);           \
-  int64_t t__ = (i) / (T_).c;                   \
-  const int x_ = (int)(t__ % (T_).w);           \
-  t__ /= (T_).w;                                \
-  const int y_ = (int)(t__ % (T_).h);           \
-  const int n_ = (int)(t__ / (T_).h)
-
 template <typename TO>
 __global__ void nchw_to_nhwc_kernel(const float* __restrict__ src, vps::TV<TO> dst, int64_t total) {
-  GRID_STRIDE(i, total) {
-    DECOMP_NHWC(i, dst, n, y, x, c);
+  VPS_GRID_STRIDE(i, total) {
+    VPS_DECOMP_NHWC(i, dst, n, y, x, c);
     vps::stf<TO>(dst.p + dst.off(n, y, x) + c, src[(((int64_t)n * dst.c + c) * dst.h + y) * dst.w + x]);
   }
 }
 template <typename TI>
 __global__ void nhwc_to_nchw_kernel(vps::TV<const TI> src, float* __restrict__ dst, int64_t total) {
-  GRID_STRIDE(i, total) {
+  VPS_GRID_STRIDE(i, total) {
     // iterate in NCHW order for coalesced writes
     const int x = (int)(i % src.w);
     int64_t t = i / src.w;
@@ -290,8 +272,8 @@ template <typename TI, typename TO>
 __global__ void im2col_kernel(vps::TV<const TI> x, vps::TV<TO> cols, int kh, int kw, int sh, int sw, int ph, int pw,
                               int64_t total) {
   const int kk = kh * kw * x.c;
-  GRID_STRIDE(i, total) {
-    DECOMP_NHWC(i, cols, n, oy, ox, k);
+  VPS_GRID_STRIDE(i, total) {
+    VPS_DECOMP_NHWC(i, cols, n, oy, ox, k);
     float v = 0.f;
     if (k < kk) {
       const int ci = k % x.c;
@@ -337,8 +319,8 @@ __global__ void im2col_bf16x8_kernel(vps::TV<const __nv_bfloat16> x, vps::TV<__n
 
 template <typename TI>
 __global__ void sigmoid_flat_kernel_t(vps::TV<const TI> src, float* __restrict__ dst, int64_t total) {
-  GRID_STRIDE(i, total) {
-    DECOMP_NHWC(i, src, n, y, x, c);
+  VPS_GRID_STRIDE(i, total) {
+    VPS_DECOMP_NHWC(i, src, n, y, x, c);
     const float v = vps::ldf<TI>(src.p + src.off(n, y, x) + c);
     dst[i] = 1.f / (1.f + expf(-v));
   }
@@ -346,19 +328,11 @@ __global__ void sigmoid_flat_kernel_t(vps::TV<const TI> src, float* __restrict__
 
 }  // namespace
 
-#define DISPATCH_IO(in_dt, out_dt, TI, TO, ...)                                                  \
-  do {                                                                                          \
-    if ((in_dt) == VPS_F32 && (out_dt) == VPS_F32) { using TI = float; using TO = float; __VA_ARGS__; }                 \
-    else if ((in_dt) == VPS_F32) { using TI = float; using TO = __nv_bfloat16; __VA_ARGS__; }                           \
-    else if ((out_dt) == VPS_F32) { using TI = __nv_bfloat16; using TO = float; __VA_ARGS__; }                          \
-    else { using TI = __nv_bfloat16; using TO = __nv_bfloat16; __VA_ARGS__; }                                           \
-  } while (0)
-
 extern "C" int vps_nchw_to_nhwc(const float* src, const vps_tensor* dst, void* stream) {
   const int64_t total = (int64_t)dst->n * dst->h * dst->w * dst->c;
   if (!total) return VPS_OK;
   VPS_DISPATCH_T(dst->dtype, TO,
-                 (nchw_to_nhwc_kernel<TO><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(src, vps::tv<TO>(*dst), total)));
+                 (nchw_to_nhwc_kernel<TO><<<vps::grid_for(total), 256, 0, (cudaStream_t)stream>>>(src, vps::tv<TO>(*dst), total)));
   VPS_CUDA_LAST("nchw_to_nhwc");
   return VPS_OK;
 }
@@ -366,7 +340,7 @@ extern "C" int vps_nhwc_to_nchw(const vps_tensor* src, float* dst, void* stream)
   const int64_t total = (int64_t)src->n * src->h * src->w * src->c;
   if (!total) return VPS_OK;
   VPS_DISPATCH_T(src->dtype, TI,
-                 (nhwc_to_nchw_kernel<TI><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(vps::tv<const TI>(*src), dst, total)));
+                 (nhwc_to_nchw_kernel<TI><<<vps::grid_for(total), 256, 0, (cudaStream_t)stream>>>(vps::tv<const TI>(*src), dst, total)));
   VPS_CUDA_LAST("nhwc_to_nchw");
   return VPS_OK;
 }
@@ -376,19 +350,10 @@ extern "C" int vps_axpby(const vps_tensor* a, const vps_tensor* b, const vps_ten
   if (b) VPS_CHECK_ARG(b->dtype == a->dtype && b->h == out->h && b->w == out->w && b->c >= out->c, "axpby: b");
   if (!((int64_t)out->n * out->h * out->w * out->c)) return VPS_OK;
   const vps_tensor bb = b ? *b : *a;
-  const bool vc = vps::vec_ok(*a, out->c) && vps::vec_ok(bb, out->c) && vps::vec_ok(*out, out->c);
-  const bool vec = a->dtype == out->dtype && vc;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (vec && out->dtype == VPS_F32)
-    axpby_kernel<float, float, 4><<<vps::pix_grid(out->w, out->c / 4, out->h, out->n), 256, 0, st>>>(
-        vps::tv<const float>(*a), vps::tv<const float>(bb), b != nullptr, vps::tv<float>(*out), alpha, beta);
-  else if (vec)
-    axpby_kernel<__nv_bfloat16, __nv_bfloat16, 8><<<vps::pix_grid(out->w, out->c / 8, out->h, out->n), 256, 0, st>>>(
-        vps::tv<const __nv_bfloat16>(*a), vps::tv<const __nv_bfloat16>(bb), b != nullptr, vps::tv<__nv_bfloat16>(*out), alpha, beta);
-  else
-    DISPATCH_IO(a->dtype, out->dtype, TI, TO,
-                (axpby_kernel<TI, TO, 1><<<vps::pix_grid(out->w, out->c, out->h, out->n), 256, 0, st>>>(
-                    vps::tv<const TI>(*a), vps::tv<const TI>(bb), b != nullptr, vps::tv<TO>(*out), alpha, beta)));
+  const bool vec = vps::vec_ok(*a, out->c) && vps::vec_ok(bb, out->c) && vps::vec_ok(*out, out->c);
+  VPS_DISPATCH_IN_OUT_V(a->dtype, out->dtype, vec, TI, TO, V,
+                        (axpby_kernel<TI, TO, V><<<vps::pix_grid(out->w, out->c / V, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(
+                            vps::tv<const TI>(*a), vps::tv<const TI>(bb), b != nullptr, vps::tv<TO>(*out), alpha, beta)));
   VPS_CUDA_LAST("axpby");
   return VPS_OK;
 }
@@ -399,18 +364,10 @@ extern "C" int vps_resize_bilinear(const vps_tensor* src, const vps_tensor* out,
   VPS_CHECK_ARG(src->c >= out->c && src->n == out->n, "resize_bilinear: shape");
   if (!((int64_t)out->n * out->h * out->w * out->c)) return VPS_OK;
   const float sy = (float)src->h / (float)out->h, sx = (float)src->w / (float)out->w;
-  const bool vec = src->dtype == out->dtype && vps::vec_ok(*src, out->c) && vps::vec_ok(*out, out->c);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (vec && out->dtype == VPS_F32)
-    resize_bilinear_kernel<float, float, 4><<<vps::pix_grid(out->w, out->c / 4, out->h, out->n), 256, 0, st>>>(
-        vps::tv<const float>(*src), vps::tv<float>(*out), sy, sx, mul);
-  else if (vec)
-    resize_bilinear_kernel<__nv_bfloat16, __nv_bfloat16, 8><<<vps::pix_grid(out->w, out->c / 8, out->h, out->n), 256, 0, st>>>(
-        vps::tv<const __nv_bfloat16>(*src), vps::tv<__nv_bfloat16>(*out), sy, sx, mul);
-  else
-    DISPATCH_IO(src->dtype, out->dtype, TI, TO,
-                (resize_bilinear_kernel<TI, TO, 1><<<vps::pix_grid(out->w, out->c, out->h, out->n), 256, 0, st>>>(
-                    vps::tv<const TI>(*src), vps::tv<TO>(*out), sy, sx, mul)));
+  const bool vec = vps::vec_ok(*src, out->c) && vps::vec_ok(*out, out->c);
+  VPS_DISPATCH_IN_OUT_V(src->dtype, out->dtype, vec, TI, TO, V,
+                        (resize_bilinear_kernel<TI, TO, V><<<vps::pix_grid(out->w, out->c / V, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(
+                            vps::tv<const TI>(*src), vps::tv<TO>(*out), sy, sx, mul)));
   VPS_CUDA_LAST("resize_bilinear");
   return VPS_OK;
 }
@@ -419,18 +376,10 @@ extern "C" int vps_resize_nearest(const vps_tensor* src, const vps_tensor* out, 
   VPS_CHECK_ARG(src->c >= out->c && src->n == out->n, "resize_nearest: shape");
   if (!((int64_t)out->n * out->h * out->w * out->c)) return VPS_OK;
   const float sy = (float)src->h / (float)out->h, sx = (float)src->w / (float)out->w;
-  const bool vec = src->dtype == out->dtype && vps::vec_ok(*src, out->c) && vps::vec_ok(*out, out->c);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (vec && out->dtype == VPS_F32)
-    resize_nearest_kernel<float, float, 4><<<vps::pix_grid(out->w, out->c / 4, out->h, out->n), 256, 0, st>>>(
-        vps::tv<const float>(*src), vps::tv<float>(*out), sy, sx, mul, accumulate);
-  else if (vec)
-    resize_nearest_kernel<__nv_bfloat16, __nv_bfloat16, 8><<<vps::pix_grid(out->w, out->c / 8, out->h, out->n), 256, 0, st>>>(
-        vps::tv<const __nv_bfloat16>(*src), vps::tv<__nv_bfloat16>(*out), sy, sx, mul, accumulate);
-  else
-    DISPATCH_IO(src->dtype, out->dtype, TI, TO,
-                (resize_nearest_kernel<TI, TO, 1><<<vps::pix_grid(out->w, out->c, out->h, out->n), 256, 0, st>>>(
-                    vps::tv<const TI>(*src), vps::tv<TO>(*out), sy, sx, mul, accumulate)));
+  const bool vec = vps::vec_ok(*src, out->c) && vps::vec_ok(*out, out->c);
+  VPS_DISPATCH_IN_OUT_V(src->dtype, out->dtype, vec, TI, TO, V,
+                        (resize_nearest_kernel<TI, TO, V><<<vps::pix_grid(out->w, out->c / V, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(
+                            vps::tv<const TI>(*src), vps::tv<TO>(*out), sy, sx, mul, accumulate)));
   VPS_CUDA_LAST("resize_nearest");
   return VPS_OK;
 }
@@ -439,18 +388,10 @@ extern "C" int vps_pool2d(const vps_tensor* src, const vps_tensor* out, int k, i
   VPS_CHECK_ARG(src->c >= out->c && src->n == out->n, "pool2d: shape");
   VPS_CHECK_ARG(out->h == (src->h + 2 * p - k) / s + 1 && out->w == (src->w + 2 * p - k) / s + 1, "pool2d: out size");
   if (!((int64_t)out->n * out->h * out->w * out->c)) return VPS_OK;
-  const bool vec = src->dtype == out->dtype && vps::vec_ok(*src, out->c) && vps::vec_ok(*out, out->c);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (vec && out->dtype == VPS_F32)
-    pool2d_kernel<float, float, 4><<<vps::pix_grid(out->w, out->c / 4, out->h, out->n), 256, 0, st>>>(
-        vps::tv<const float>(*src), vps::tv<float>(*out), k, s, p, is_avg);
-  else if (vec)
-    pool2d_kernel<__nv_bfloat16, __nv_bfloat16, 8><<<vps::pix_grid(out->w, out->c / 8, out->h, out->n), 256, 0, st>>>(
-        vps::tv<const __nv_bfloat16>(*src), vps::tv<__nv_bfloat16>(*out), k, s, p, is_avg);
-  else
-    DISPATCH_IO(src->dtype, out->dtype, TI, TO,
-                (pool2d_kernel<TI, TO, 1><<<vps::pix_grid(out->w, out->c, out->h, out->n), 256, 0, st>>>(
-                    vps::tv<const TI>(*src), vps::tv<TO>(*out), k, s, p, is_avg)));
+  const bool vec = vps::vec_ok(*src, out->c) && vps::vec_ok(*out, out->c);
+  VPS_DISPATCH_IN_OUT_V(src->dtype, out->dtype, vec, TI, TO, V,
+                        (pool2d_kernel<TI, TO, V><<<vps::pix_grid(out->w, out->c / V, out->h, out->n), 256, 0, (cudaStream_t)stream>>>(
+                            vps::tv<const TI>(*src), vps::tv<TO>(*out), k, s, p, is_avg)));
   VPS_CUDA_LAST("pool2d");
   return VPS_OK;
 }
@@ -477,33 +418,26 @@ extern "C" int vps_groupnorm(const vps_tensor* x, const vps_tensor* y, const flo
   int chunks = (int)((per_group + 256 * 32 - 1) / (256 * 32));
   if (chunks > 64) chunks = 64;
   if (chunks < 1) chunks = 1;
-  const int V = x->dtype == VPS_F32 ? 4 : 8;
   const int cg = x->c / groups;
-  const bool vstats = vps::vec_ok(*x, x->c) && (x->c / V) <= 256 && 256 % (x->c / V) == 0 && (cg >= V ? cg % V == 0 : V == 2 * cg);
-  if (vstats) {
-    const int rows = 256 / (x->c / V);
-    int64_t slices = ((int64_t)x->h * x->w + rows * 32 - 1) / (rows * 32);
-    if (slices > 148 * 4) slices = 148 * 4;
-    if (slices < 1) slices = 1;
-    dim3 grid((unsigned)slices, 1, x->n);
-    if (x->dtype == VPS_F32) gn_stats_vec_kernel<float, 4><<<grid, 256, 0, st>>>(vps::tv<const float>(*x), groups, g_gn_stats);
-    else gn_stats_vec_kernel<__nv_bfloat16, 8><<<grid, 256, 0, st>>>(vps::tv<const __nv_bfloat16>(*x), groups, g_gn_stats);
-  } else {
-    dim3 grid(chunks, groups, x->n);
-    VPS_DISPATCH_T(x->dtype, TI, (gn_stats_kernel<TI><<<grid, 256, 0, st>>>(vps::tv<const TI>(*x), groups, g_gn_stats)));
-  }
+  VPS_DISPATCH_T(x->dtype, TI, {
+    constexpr int V = vps::VecW<TI>::value;
+    if (vps::vec_ok(*x, x->c) && (x->c / V) <= 256 && 256 % (x->c / V) == 0 && (cg >= V ? cg % V == 0 : V == 2 * cg)) {
+      const int rows = 256 / (x->c / V);
+      int64_t slices = ((int64_t)x->h * x->w + rows * 32 - 1) / (rows * 32);
+      if (slices > 148 * 4) slices = 148 * 4;
+      if (slices < 1) slices = 1;
+      dim3 grid((unsigned)slices, 1, x->n);
+      gn_stats_vec_kernel<TI, V><<<grid, 256, 0, st>>>(vps::tv<const TI>(*x), groups, g_gn_stats);
+    } else {
+      dim3 grid(chunks, groups, x->n);
+      gn_stats_kernel<TI><<<grid, 256, 0, st>>>(vps::tv<const TI>(*x), groups, g_gn_stats);
+    }
+  });
   VPS_CUDA_LAST("gn_stats");
-  const bool vec = x->dtype == y->dtype && vps::vec_ok(*x, x->c) && vps::vec_ok(*y, x->c);
-  if (vec && y->dtype == VPS_F32)
-    gn_apply_kernel<float, float, 4><<<vps::pix_grid(y->w, y->c / 4, y->h, y->n), 256, 0, st>>>(
-        vps::tv<const float>(*x), vps::tv<float>(*y), g_gn_stats, gamma, beta, groups, eps, relu);
-  else if (vec)
-    gn_apply_kernel<__nv_bfloat16, __nv_bfloat16, 8><<<vps::pix_grid(y->w, y->c / 8, y->h, y->n), 256, 0, st>>>(
-        vps::tv<const __nv_bfloat16>(*x), vps::tv<__nv_bfloat16>(*y), g_gn_stats, gamma, beta, groups, eps, relu);
-  else
-    DISPATCH_IO(x->dtype, y->dtype, TI, TO,
-                (gn_apply_kernel<TI, TO, 1><<<vps::pix_grid(y->w, y->c, y->h, y->n), 256, 0, st>>>(
-                    vps::tv<const TI>(*x), vps::tv<TO>(*y), g_gn_stats, gamma, beta, groups, eps, relu)));
+  const bool vec = vps::vec_ok(*x, x->c) && vps::vec_ok(*y, x->c);
+  VPS_DISPATCH_IN_OUT_V(x->dtype, y->dtype, vec, TI, TO, V,
+                        (gn_apply_kernel<TI, TO, V><<<vps::pix_grid(y->w, y->c / V, y->h, y->n), 256, 0, st>>>(
+                            vps::tv<const TI>(*x), vps::tv<TO>(*y), g_gn_stats, gamma, beta, groups, eps, relu)));
   VPS_CUDA_LAST("gn_apply");
   return VPS_OK;
 }
@@ -525,9 +459,9 @@ extern "C" int vps_im2col(const vps_tensor* x, const vps_tensor* cols, int kh, i
     VPS_CUDA_LAST("im2col_bf16x8");
     return VPS_OK;
   }
-  DISPATCH_IO(x->dtype, cols->dtype, TI, TO,
-              (im2col_kernel<TI, TO><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(
-                  vps::tv<const TI>(*x), vps::tv<TO>(*cols), kh, kw, sh, sw, ph, pw, total)));
+  VPS_DISPATCH_T(x->dtype, TI, VPS_DISPATCH_T(cols->dtype, TO,
+      (im2col_kernel<TI, TO><<<vps::grid_for(total), 256, 0, (cudaStream_t)stream>>>(
+          vps::tv<const TI>(*x), vps::tv<TO>(*cols), kh, kw, sh, sw, ph, pw, total))));
   VPS_CUDA_LAST("im2col");
   return VPS_OK;
 }
@@ -538,7 +472,7 @@ extern "C" int vps_sigmoid_flat(const vps_tensor* t, float* dst, void* stream) {
   const int64_t total = (int64_t)t->n * t->h * t->w * t->c;
   if (!total) return VPS_OK;
   VPS_DISPATCH_T(t->dtype, TI,
-                 (sigmoid_flat_kernel_t<TI><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(vps::tv<const TI>(*t), dst, total)));
+                 (sigmoid_flat_kernel_t<TI><<<vps::grid_for(total), 256, 0, (cudaStream_t)stream>>>(vps::tv<const TI>(*t), dst, total)));
   VPS_CUDA_LAST("sigmoid_flat");
   return VPS_OK;
 }
@@ -552,9 +486,9 @@ extern "C" int vps_space_to_depth2(const vps_tensor* x, const vps_tensor* y, voi
     VPS_CUDA_LAST("space_to_depth2");
     return VPS_OK;
   }
-  DISPATCH_IO(x->dtype, y->dtype, TI, TO,
-              (space_to_depth2_kernel<TI, TO><<<vps::pix_grid(y->w, y->c, y->h, y->n), 256, 0, (cudaStream_t)stream>>>(
-                  vps::tv<const TI>(*x), vps::tv<TO>(*y))));
+  VPS_DISPATCH_T(x->dtype, TI, VPS_DISPATCH_T(y->dtype, TO,
+      (space_to_depth2_kernel<TI, TO><<<vps::pix_grid(y->w, y->c, y->h, y->n), 256, 0, (cudaStream_t)stream>>>(
+          vps::tv<const TI>(*x), vps::tv<TO>(*y)))));
   VPS_CUDA_LAST("space_to_depth2");
   return VPS_OK;
 }
