@@ -89,6 +89,13 @@ int vps_conv2d_tc(const vps_conv_args* a, void* stream);
 /* up to 4 problems sharing x / y / geometry / bias / activation and differing in w, (ph,pw) and (oy_off,ox_off):
  * the stride phases of a ConvTranspose2d (submodules.py:33-37, fcn_mask_head.py:66-71) in one persistent launch. */
 int vps_conv2d_tc_multi(const vps_conv_args* a, int nprob, void* stream);
+/* The tiling vps_conv2d_tc_multi(a, nprob) launches, from the shapes in `a` and the current device's SM count (no pointer
+ * is read): plan[0] = block_n (output channels per tile), plan[1] = tile width, plan[2] = tile height (output pixels),
+ * plan[3] = 1 in halo mode (stride 1, > 1 tap: one activation box per channel chunk feeds every tap), plan[4] = rowg (halo
+ * mode: 1 = one weight ring slot holds the kw taps of a filter row), plan[5] = gsub (flat mode: K steps per ring slot),
+ * plan[6] = bk (channels per K step, 64 or 16), plan[7] / plan[8] = slots of the activation / weight rings (equal in flat
+ * mode, where one ring holds both), plan[9] = tiles of the launch (over all problems).  `plan` holds 10 ints. */
+int vps_conv2d_tc_plan(const vps_conv_args* a, int nprob, int* plan);
 int vps_conv2d_simt(const vps_conv_args* a, void* stream);
 /* OIHW fp32 (torch layout, on device) -> packed layouts.  scale[cout] (may be NULL) is folded in
  * (frozen BatchNorm: resnet.py:519-526).  transposed != 0: src is IOHW (ConvTranspose2d). */

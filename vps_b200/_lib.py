@@ -67,7 +67,7 @@ def check(status, what=""):
 # every symbol include/vps_b200.h declares (tests assert the .so exports all of them)
 EXPORTS = [
     "vps_last_error", "vps_version", "vps_launch_count", "vps_add_launch_count",
-    "vps_conv2d_tc", "vps_conv2d_tc_multi", "vps_conv2d_simt", "vps_pack_weights_tc", "vps_pack_weights_simt",
+    "vps_conv2d_tc", "vps_conv2d_tc_multi", "vps_conv2d_tc_plan", "vps_conv2d_simt", "vps_pack_weights_tc", "vps_pack_weights_simt",
     "vps_packed_tc_bytes", "vps_im2col",
     "vps_conv2d_tc32", "vps_conv2d_tc32_multi", "vps_conv2d_tc32_plan", "vps_pack_weights_tc32", "vps_packed_tc32_bytes", "vps_tc32_overflow", "vps_deform_conv_tc32", "vps_deform_conv_tc32_plan",
     "vps_correlation", "vps_correlation_tc", "vps_correlation_simt", "vps_correlation_tc32", "vps_correlation_tc32_ws_bytes", "vps_resample2d", "vps_channelnorm", "vps_flownet_input", "vps_flownet_stage", "vps_flownet_cat3", "vps_flow_deconv",

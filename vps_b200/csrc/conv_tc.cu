@@ -457,28 +457,15 @@ extern "C" int vps_pack_weights_tc(const float* w, const float* scale, void* dst
   return VPS_OK;
 }
 
-// nprob problems (<= 4) that share x / y / geometry / epilogue and differ in weights, padding and output pixel
-// offset: the four stride phases of a transposed convolution run as ONE persistent launch.
-extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* stream) {
+// The tiling and rings of vps_conv2d_tc_multi(a, nprob), from the shapes in `a` and the current device's SM count (no pointer
+// is read); set_problems() adds the output, residual and epilogue.
+static int tc_plan(const vps_conv_args* a, int nprob, ConvTcParams& p) {
   VPS_CHECK_ARG(nprob >= 1 && nprob <= MAX_PROB, "conv2d_tc: nprob %d", nprob);
-  const vps_conv_args* a = &args[0];
-  VPS_CHECK_ARG(a->x.dtype == VPS_BF16, "conv2d_tc: x must be bf16");
-  VPS_CHECK_ARG(a->x.cs % 8 == 0 && ((uintptr_t)a->x.ptr & 15) == 0, "conv2d_tc: x not 16B aligned (cs=%d)",
-                a->x.cs);
   VPS_CHECK_ARG(a->sh >= 1 && a->sh <= 2 && a->sw >= 1 && a->sw <= 2, "conv2d_tc: stride must be 1 or 2");
-  VPS_CHECK_ARG(a->cin == a->x.c, "conv2d_tc: cin %d != x.c %d", a->cin, a->x.c);
-  for (int i = 0; i < nprob; ++i) {
-    VPS_CHECK_ARG(((uintptr_t)args[i].w & 15) == 0, "conv2d_tc: weights not aligned");
-    VPS_CHECK_ARG(args[i].x.ptr == a->x.ptr && args[i].y.ptr == a->y.ptr && args[i].kh == a->kh && args[i].kw == a->kw &&
-                      args[i].oh == a->oh && args[i].ow == a->ow && args[i].cout == a->cout && args[i].bias == a->bias &&
-                      args[i].act == a->act && args[i].oy_mul == a->oy_mul && args[i].ox_mul == a->ox_mul &&
-                      args[i].cin_gran == a->cin_gran,
-                  "conv2d_tc_multi: problems must share geometry");
-  }
   const int sms = vps::num_sms();
   if (sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
 
-  ConvTcParams p = {};
+  p = {};
   const int bk = a->cin_gran == 16 ? 16 : 64;
   p.bk = bk;
   const int cin_pad = cin_pad_for(a->cin, bk);
@@ -541,24 +528,57 @@ extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* s
     if (stages > MAX_STAGES) stages = MAX_STAGES;
     p.a_stages = p.b_stages = stages;
   }
-  const int st = set_problems(p, args, nprob, "conv2d_tc");
+  return VPS_OK;
+}
+
+// nprob problems (<= 4) that share x / y / geometry / epilogue and differ in weights, padding and output pixel
+// offset: the four stride phases of a transposed convolution run as ONE persistent launch.
+extern "C" int vps_conv2d_tc_multi(const vps_conv_args* args, int nprob, void* stream) {
+  VPS_CHECK_ARG(nprob >= 1 && nprob <= MAX_PROB, "conv2d_tc: nprob %d", nprob);
+  const vps_conv_args* a = &args[0];
+  VPS_CHECK_ARG(a->x.dtype == VPS_BF16, "conv2d_tc: x must be bf16");
+  VPS_CHECK_ARG(a->x.cs % 8 == 0 && ((uintptr_t)a->x.ptr & 15) == 0, "conv2d_tc: x not 16B aligned (cs=%d)",
+                a->x.cs);
+  VPS_CHECK_ARG(a->cin == a->x.c, "conv2d_tc: cin %d != x.c %d", a->cin, a->x.c);
+  for (int i = 0; i < nprob; ++i) {
+    VPS_CHECK_ARG(((uintptr_t)args[i].w & 15) == 0, "conv2d_tc: weights not aligned");
+    VPS_CHECK_ARG(args[i].x.ptr == a->x.ptr && args[i].y.ptr == a->y.ptr && args[i].kh == a->kh && args[i].kw == a->kw &&
+                      args[i].oh == a->oh && args[i].ow == a->ow && args[i].cout == a->cout && args[i].bias == a->bias &&
+                      args[i].act == a->act && args[i].oy_mul == a->oy_mul && args[i].ox_mul == a->ox_mul &&
+                      args[i].cin_gran == a->cin_gran,
+                  "conv2d_tc_multi: problems must share geometry");
+  }
+  ConvTcParams p;
+  int st = tc_plan(a, nprob, p);
+  if (st != VPS_OK) return st;
+  st = set_problems(p, args, nprob, "conv2d_tc");
   if (st != VPS_OK) return st;
   if (p.total_tiles == 0) return VPS_OK;
 
+  const int bk = p.bk, halo_h = p.th + a->kh - 1;
   CUtensorMap tmA, tmB[MAX_PROB];
-  if (!vps::encode_nhwc(&tmA, a->x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, bk, halo ? p.halo_w : tw * a->sw, halo ? halo_h : th * a->sh,
+  if (!vps::encode_nhwc(&tmA, a->x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, bk, p.halo ? p.halo_w : p.tw * a->sw, p.halo ? halo_h : p.th * a->sh,
                         a->sw, a->sh, bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_32B,
                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "conv2d_tc: encode A"))
     return VPS_E_CUDA;
   for (int i = 0; i < MAX_PROB; ++i)
-    if (!encode_weights_tc(&tmB[i], args[i < nprob ? i : 0].w, a->cout, a->kh * a->kw, cin_pad, bk, block_n, p.rowg ? a->kw : 1,
-                           "conv2d_tc"))
+    if (!encode_weights_tc(&tmB[i], args[i < nprob ? i : 0].w, a->cout, a->kh * a->kw, cin_pad_for(a->cin, bk), bk, p.block_n,
+                           p.rowg ? a->kw : 1, "conv2d_tc"))
       return VPS_E_CUDA;
   return launch_persistent<conv_igemm_tc_kernel>(p.total_tiles, NUM_THREADS, (int)tc_ring(0, p, false).smem, stream, "conv2d_tc",
                                                  tmA, tmB[0], tmB[1], tmB[2], tmB[3], p);
 }
 
 extern "C" int vps_conv2d_tc(const vps_conv_args* a, void* stream) { return vps_conv2d_tc_multi(a, 1, stream); }
+
+extern "C" int vps_conv2d_tc_plan(const vps_conv_args* a, int nprob, int* plan) {
+  ConvTcParams p;
+  const int st = tc_plan(a, nprob, p);
+  if (st != VPS_OK) return st;
+  const int v[10] = {p.block_n, p.tw, p.th, p.halo, p.rowg, p.gsub, p.bk, p.a_stages, p.b_stages, p.total_tiles};
+  for (int i = 0; i < 10; ++i) plan[i] = v[i];
+  return VPS_OK;
+}
 
 
 // Fused DCNv1 3x3 / stride 1 / pad 1 / dilation 1 / 1 deformable group (deform_conv.py:15-87 forward):

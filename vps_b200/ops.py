@@ -284,6 +284,24 @@ def conv2d_tc32_plan(x, pws, stride=1, pad=0, oh=None, ow=None, pads=None, y=Non
     return dict(nwg=plan[0], block_n=plan[1], tw=plan[2], th=plan[3], halo=plan[4], epilogue="tma" if plan[5] else "frag")
 
 
+def conv2d_tc_plan(x, pws, stride=1, pad=0, oh=None, ow=None, pads=None, y=None, res=None, omaps=None):
+    """The tiling the bf16 tensor-core kernel picks for conv2d (one problem) or conv2d_tc_multi (`pads` = per-phase
+    (ph, pw), stride 1, `omaps` = per-phase output maps): dict(block_n, tw, th (output pixels per tile), halo, rowg (halo
+    mode: the taps of a filter row share a weight ring slot), gsub (flat mode: K steps per ring slot), bk (channels per K
+    step), a_stages, b_stages (ring slots), total_tiles)."""
+    pws = pws if isinstance(pws, (list, tuple)) else [pws]
+    n = len(pws)
+    arr = (VpsConvArgs * n)()
+    for i in range(n):
+        arr[i] = _conv_args(x, pws[i], x if y is None else y, stride, pad, ACT_NONE, 0.1, res, False, 1.0, oh, ow,
+                            omaps[i] if omaps is not None else (1, 0, 1, 0), pads[i] if pads is not None else None)
+        arr[i].cin_gran = pws[0].gran()
+    plan = (C.c_int * 10)()
+    check(_real_lib().vps_conv2d_tc_plan(arr, n, plan), "conv2d_tc_plan")
+    keys = ("block_n", "tw", "th", "halo", "rowg", "gsub", "bk", "a_stages", "b_stages", "total_tiles")
+    return dict(zip(keys, plan))
+
+
 # ------------------------------------------------------------------ FlowNet2 native ops
 def correlation(f1, f2, out, pad, max_disp, stride1, stride2, act=ACT_NONE, slope=0.1, impl=None):
     """impl: None = dispatch (tensor cores for bf16 features, and for fp32 features in the tc32 precision), "tc" / "tc32" /
