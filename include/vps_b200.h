@@ -121,11 +121,14 @@ int64_t vps_packed_tc_bytes(int cout, int cin, int kh, int kw, int cin_gran);
 int vps_conv2d_tc32(const vps_conv_args* a, void* stream);
 int vps_conv2d_tc32_multi(const vps_conv_args* a, int nprob, void* stream);
 /* The tiling vps_conv2d_tc32_multi(a, nprob) launches, from the shapes in `a` and the current device's SM count (no
- * pointer is read): plan[0] = consumer warpgroups (2: 128-pixel tiles, block_n <= 128; 4: 256-pixel tiles, block_n <= 64),
- * plan[1] = block_n, plan[2] = tile width, plan[3] = tile height (output pixels), plan[4] = 1 in halo mode (stride 1,
- * > 1 tap: one activation box per 32-channel chunk feeds every tap), plan[5] = 1 for the TMA epilogue (results staged in
- * shared memory and stored by TMA; one fp32 problem with 16-byte aligned output / residual slices, block_n <= 64, and
- * room in shared memory), 0 for stores straight from the accumulator fragments.  `plan` holds 6 ints. */
+ * pointer is read): plan[0] = consumer warpgroups NWG (2: up to 128 channels per warpgroup; 4: up to 64), plan[1] =
+ * block_n (channels per tile), plan[2] = tile width, plan[3] = tile height (output pixels), plan[4] = 1 in halo mode
+ * (stride 1, > 1 tap: one activation box per 32-channel chunk feeds every tap), plan[5] = 1 for the TMA epilogue (results
+ * staged in shared memory and stored by TMA; one fp32 problem with 16-byte aligned output / residual slices, <= 64
+ * channels per warpgroup, and room in shared memory), 0 for stores straight from the accumulator fragments, plan[6] = Q,
+ * the channel groups of the layout (P, Q), P * Q = NWG: the tile holds 64 P pixels, and warpgroup w takes pixels
+ * 64 (w / Q) .. + 63 and channels (block_n / Q) (w % Q) .. of it, all warpgroups sharing the tile's converted activations
+ * and weight tile.  `plan` holds 7 ints. */
 int vps_conv2d_tc32_plan(const vps_conv_args* a, int nprob, int* plan);
 int vps_pack_weights_tc32(const float* w_oihw, const float* scale, void* dst, int cout, int cin, int kh, int kw,
                           int transposed, int prob, int nprob, void* stream);

@@ -49,6 +49,12 @@ DECONVS = [
 flush = None
 
 
+def plan_str(plan):
+    """nwg, layout (P pixel groups x Q channel groups), channels per warpgroup, epilogue"""
+    return "nwg %d layout %dx%d bn %d/wg %s" % (plan["nwg"], plan["layout"][0], plan["layout"][1], plan["block_n"] // plan["wg_n"],
+                                                 plan["epilogue"])
+
+
 def timeit(fn, iters=5):
     fn()
     torch.cuda.synchronize()
@@ -91,8 +97,8 @@ def main():
         fl = 2.0 * n * oh * ow * cout * cin * k * k
         by = 4.0 * n * (h * w * cin + oh * ow * cout * (2 if res else 1))
         print("%-28s %dx%d s%d %4d->%4d @%dx%d n%d: %.4f ms  %6.1f TF/s alg  %6.1f MB  hbm-floor %.4f ms (%.2f of it)  "
-              "nwg %d bn %d %s" % (note, k, k, s, cin, cout, oh, ow, n, ms, fl / ms / 1e9, by / 1e6, by / HBM_GBPS / 1e6,
-                                   by / HBM_GBPS / 1e6 / ms, plan["nwg"], plan["block_n"], plan["epilogue"]), flush=True)
+              "%s" % (note, k, k, s, cin, cout, oh, ow, n, ms, fl / ms / 1e9, by / 1e6, by / HBM_GBPS / 1e6,
+                      by / HBM_GBPS / 1e6 / ms, plan_str(plan)), flush=True)
         del x, y, r, pk
     from vps_b200.layers import deconv4x4_s2
     for (n, cin, cout, h, w, note) in DECONVS:
@@ -104,10 +110,12 @@ def main():
         layer = deconv4x4_s2((torch.randn(cin, cout, 4, 4, generator=g) / (cin * 4) ** 0.5).to(dev),
                              torch.randn(cout, generator=g).to(dev))
         y = empty_nhwc(n, 2 * h, 2 * w, cout, torch.float32, dev)
+        plan = ops.conv2d_tc32_plan(x, [ph[3] for ph in layer.phases], pads=[ph[2] for ph in layer.phases], oh=h, ow=w, y=y,
+                                    omaps=[(2, ph[0], 2, ph[1]) for ph in layer.phases])
         ms = timeit(lambda: layer(x, y, act=ops.ACT_LRELU))
         fl = 2.0 * n * h * w * cout * cin * 16
-        print("%-28s 2x2 x4 phases %4d->%4d @%dx%d n%d: %.4f ms  %6.1f TF/s alg" % (note, cin, cout, h, w, n, ms, fl / ms / 1e9),
-              flush=True)
+        print("%-28s 2x2 x4 phases %4d->%4d @%dx%d n%d: %.4f ms  %6.1f TF/s alg  %s" % (note, cin, cout, h, w, n, ms, fl / ms / 1e9,
+                                                                                       plan_str(plan)), flush=True)
         del x, y, layer
     if "--dcn" in sys.argv:
         for (h, w) in [(256, 512), (128, 256), (64, 128), (32, 64)]:

@@ -22,21 +22,24 @@
 //     main product A*B is added on top -- a chain of 2 main MMAs;
 //   * that step result is promoted into a per-thread register sum with a round-to-nearest fp32 add.
 //
-// Pipeline per CTA (persistent, one (64 * NWG)-pixel x block_n tile at a time, K consumed 32 channels per step):
+// Pipeline per CTA (persistent, one (64 * P)-pixel x block_n tile at a time, K consumed 32 channels per step):
 //   warp 0          : TMA producer: raw fp32 activation boxes {32 ch, pixels} into a staging ring; pre-split weight tiles
 //                     [B | B2] (vps_pack_weights_tc32) into the B ring.
 //   warps 1-3       : converters: staging box -> two SWIZZLE_64B operand planes A, A2 (generic-proxy writes ->
 //                     fence.proxy.async -> mbarrier).  In halo mode (stride 1, > 1 tap) one converted (th+kh-1) x (tw+kw-1)
 //                     box feeds all kh*kw taps through shifted descriptor start addresses.
-//   warpgroups 1..NWG: consumers, pixels 64 wg .. 64 wg + 63: wgmma.kind f16 (M64 x N x K16) into registers, promotion, then
-//                     bias / activation / residual and the NHWC store.  Flat tiles (block_n <= 64, aligned fp32 output)
-//                     stage the result in shared-memory output boxes and store them by TMA while the next tile's K steps
-//                     run, the residual having arrived by TMA during the K steps; halo tiles and outputs no tensor map
-//                     expresses store straight from the accumulator fragments.
-// NWG = 2 (384 threads, block_n <= 128) or 4 (640 threads, block_n <= 64).  A K step is two dependent wgmma round trips
-// (the promotion order above), so a warpgroup spends a fixed few hundred clocks per step whatever N is; at N <= 64 four
-// warpgroups overlap those round trips and share each converted box and weight tile among twice the pixels.  At 640
-// threads the register cap is 96, which holds the N = 64 step accumulator + sum.  vps_conv2d_tc32_plan picks NWG.
+//   warpgroups 1..NWG: consumers: wgmma.kind f16 (M64 x N x K16) into registers, promotion, then bias / activation /
+//                     residual and the NHWC store.  Flat tiles (N <= 64, aligned fp32 output) stage the result in
+//                     shared-memory output boxes and store them by TMA while the next tile's K steps run, the residual
+//                     having arrived by TMA during the K steps; halo tiles and outputs no tensor map expresses store straight
+//                     from the accumulator fragments.
+// Layout (P, Q), P * Q = NWG: the tile holds 64 P pixels x block_n = Q N channels, and consumer warpgroup w takes pixels
+// 64 (w / Q) .. + 63 and channels N (w % Q) .. + N - 1 of it (Tc32Share).  All NWG warpgroups read the one converted box and
+// the one weight tile of a step.  NWG = 2 (384 threads, N <= 128): (2, 1); NWG = 4 (640 threads, N <= 64): (4, 1), and
+// (2, 2), (1, 4) at N = 64 (tc32_plan).  A K step is two dependent wgmma round trips (the promotion order above), so a warpgroup spends a few
+// hundred clocks per step however small N is; four warpgroups overlap those round trips, and Q > 1 lets them do so on
+// layers of 128 and more channels without converting the same activations once per N tile.  At 640 threads the register
+// cap is 96, which holds the N = 64 step accumulator + sum.  vps_conv2d_tc32_plan picks (NWG, Q, N).
 #include "conv_tc_common.cuh"
 
 namespace {
@@ -53,13 +56,22 @@ constexpr int T32_PLANES = 2;               // operand planes: fp16(v), fp16(2^1
 __device__ unsigned int g_tc32_overflow = 0;     // activations / weights that exceeded the fp16 range of the main product
 
 struct Tc32Extra {
-  int rows;                  // activation rows (pixels) per A item: halo_h * halo_w, or the tile's 64 * NWG pixels
+  int rows;                  // activation rows (pixels) per A item: halo_h * halo_w, or the tile's 64 * P pixels
   int plane_bytes;           // bytes of one operand plane of an A item (rows * 64, padded to 1024)
   int stage_bytes;           // bytes of one fp32 staging slot (rows * 128, padded to 1024)
   int b_plane_bytes;         // block_n * 64: one weight plane of one step
   int dcn;                   // 1: the operand planes are produced by the deformable-sampling warps (no activation TMA)
-  int dcn_split_n;           // DCN split-N layout: the consumer warpgroups share the tile's pixels, each takes block_n / 2 channels
+  int wg_n;                  // Q: channel groups of consumer warpgroups; each warpgroup takes block_n / Q of the tile's channels
 };
+
+// Consumer warpgroup wg's share of a tile: pixels row0 .. row0 + 63, channels c_off .. c_off + n - 1 (n = block_n / Q).
+struct Tc32Share {
+  int row0, c_off, n;
+};
+__host__ __device__ __forceinline__ Tc32Share tc32_share(const ConvTcParams& p, const Tc32Extra& e, int wg) {
+  const int n = p.block_n / e.wg_n, lg = e.wg_n >> 1;    // Q is 1, 2 or 4: shifts, not divisions, in the epilogue
+  return {64 * (wg >> lg), n * (wg & (e.wg_n - 1)), n};
+}
 
 // the fused DCN kernel is bound by its sampling warps (CUDA-core issue + L1 latency), so it runs 4 warpgroups: warp 0 = weight
 // TMA, warps 1-3 and 12-15 = 7 sampling warps, warpgroups 1 and 2 = consumers.  setmaxnreg moves registers from warpgroups 0
@@ -105,17 +117,19 @@ constexpr int t32_box_c(int n) { return n >= 32 ? 32 : 16; }
 constexpr int T32_EPI_MAX_N = 64;
 
 // Shared memory of the tc32 kernels from the 1024-byte aligned `base`, in this order: the convolution's staging ring,
-// operand-plane ring, weight ring, with the TMA epilogue the output boxes and bias of the nwg consumer warpgroups, the DCN's
-// set-up table, then the barriers.  The ring slots are multiples of 1 KB, so every region after them is 1024-byte aligned.
+// operand-plane ring, weight ring, with the TMA epilogue the 64 x N output boxes and N bias values of each of the nwg consumer
+// warpgroups, the DCN's set-up table, then the barriers.  The ring slots are multiples of 1 KB, so every region after them is
+// 1024-byte aligned.
 __host__ __device__ __forceinline__ Ring32 ring32(uint32_t base, const ConvTcParams& p, const Tc32Extra& e, int nwg, bool epi_tma,
                                                   bool dcn) {
   Ring32 rg;
+  const uint32_t n = (uint32_t)(p.block_n / e.wg_n);
   rg.s_base = base; rg.s_bytes = dcn ? 0u : (uint32_t)e.stage_bytes;
   rg.a_base = rg.s_base + T32_STAGE_SLOTS * rg.s_bytes; rg.a_bytes = (uint32_t)T32_PLANES * (uint32_t)e.plane_bytes;
   rg.b_base = rg.a_base + (uint32_t)p.a_stages * rg.a_bytes; rg.b_bytes = (uint32_t)T32_PLANES * (uint32_t)e.b_plane_bytes;
   rg.e_base = rg.b_base + (uint32_t)p.b_stages * rg.b_bytes;
-  rg.bias_base = rg.e_base + (epi_tma ? 64u * nwg * (uint32_t)p.block_n * 4u : 0u);
-  rg.setup_base = rg.bias_base + (epi_tma ? (uint32_t)nwg * (uint32_t)p.block_n * 4u : 0u);
+  rg.bias_base = rg.e_base + (epi_tma ? 64u * nwg * n * 4u : 0u);
+  rg.setup_base = rg.bias_base + (epi_tma ? (uint32_t)nwg * n * 4u : 0u);
   rg.bar_base = rg.setup_base + (dcn ? (uint32_t)dcn_setup_bytes(e.rows) : 0u);
   rg.smem = rg.bar_base + T32_BAR_BYTES + 1024u - base;
   return rg;
@@ -302,17 +316,18 @@ __device__ __forceinline__ uint32_t epi_box_addr(uint32_t box, int q, int c) {
   return box + (uint32_t)(c / BC) * (64u * BC * 4u) + (uint32_t)q * (BC * 4u) + ((k ^ sw) << 4) + (uint32_t)(c & 3) * 4u;
 }
 
-// The output box of warpgroup wg in tile `tile`: channels n0.., pixels (x0, y0).. of image img; live = any pixel in range.
-// Recomputed where it is needed rather than held in registers across the K steps.
+// The output box of warpgroup wg in tile `tile` (its tc32_share): channels n0.., pixels (x0, y0).. of image img; live = any
+// pixel in range.  Recomputed where it is needed rather than held in registers across the K steps.
 struct EpiBox {
   int n0, x0, y0, img;
   bool live;
 };
-__device__ __forceinline__ EpiBox epi_box(const ConvTcParams& p, int tile, int wg) {
+__device__ __forceinline__ EpiBox epi_box(const ConvTcParams& p, const Tc32Extra& e, int tile, int wg) {
   const TileCoord t = tile_coord(p, tile);
+  const Tc32Share s = tc32_share(p, e, wg);
   EpiBox b;
-  b.n0 = t.n_idx * p.block_n; b.img = t.img;
-  b.x0 = t.tx * p.tw + (64 * wg) % p.tw; b.y0 = t.ty * p.th + (64 * wg) / p.tw;
+  b.n0 = t.n_idx * p.block_n + s.c_off; b.img = t.img;
+  b.x0 = t.tx * p.tw + s.row0 % p.tw; b.y0 = t.ty * p.th + s.row0 / p.tw;
   b.live = b.x0 < p.ow && b.y0 < p.oh;
   return b;
 }
@@ -321,7 +336,7 @@ __device__ __forceinline__ EpiBox epi_box(const ConvTcParams& p, int tile, int w
 // filled) -> TMA store of the boxes.  The store stays in flight while the warpgroup runs the next tile's K steps.  The
 // boxes are written again only after the leader's cp.async.bulk.wait_group.read, i.e. once the store has read them.
 template <int N>
-__device__ __forceinline__ void epi_tma32(const ConvTcParams& p, const CUtensorMap* tmY, const float (&d)[N / 2], uint32_t box,
+__device__ __forceinline__ void epi_tma32(const ConvTcParams& p, const Tc32Extra& e, const CUtensorMap* tmY, const float (&d)[N / 2], uint32_t box,
                                           uint32_t bias_s, float bias_v, uint32_t rbar, uint32_t rphase, int wg, int tile) {
   constexpr int BC = t32_box_c(N);
   const int i = threadIdx.x & 127, lane = threadIdx.x & 31, w = i >> 5;
@@ -345,7 +360,7 @@ __device__ __forceinline__ void epi_tma32(const ConvTcParams& p, const CUtensorM
   }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");        // generic-proxy writes -> TMA reads
   asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-  const EpiBox eb = epi_box(p, tile, wg);
+  const EpiBox eb = epi_box(p, e, tile, wg);
   if (i == 0 && eb.live) {
 #pragma unroll
     for (int b = 0; b < N / BC; ++b) tma_store_4d(tmY, box + (uint32_t)b * (64u * BC * 4u), eb.n0 + b * BC, eb.x0, eb.y0, eb.img);
@@ -358,14 +373,17 @@ __device__ __forceinline__ void epi_tma32(const ConvTcParams& p, const CUtensorM
 // and weight tiles of the step are released as soon as its MMAs have completed (one arrival per consumer warpgroup).
 // With the TMA epilogue the leader loads the tile's residual boxes after the first K step: by then the previous tile's store
 // has long read the boxes, so its wait does not hold up the first MMAs.
-// The warpgroup's share of the tile: pixels row0 .. row0 + 63, the N weight rows from byte b_off of each weight plane, tile
-// channels c_off .. c_off + N - 1 (the convolution: 64 wg, 0, 0).
+// The warpgroup's share of the tile (tc32_share, N = its channel count): pixels row0 .. row0 + 63, tile channels
+// c_off .. c_off + N - 1, whose weight rows start at byte c_off * 64 of each weight plane.  The epilogue recomputes the share
+// rather than holding it in registers across the K steps.
 template <int N, bool TMA_EPI>
-__device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, int wg, int row0,
-                                           uint32_t b_off, int c_off, const CUtensorMap* tmY, const CUtensorMap* tmR) {
+__device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, int wg, const CUtensorMap* tmY,
+                                           const CUtensorMap* tmR) {
   constexpr int BC = t32_box_c(N);
   const bool leader = (threadIdx.x & 127) == 0;
   constexpr bool epi_tma = TMA_EPI;
+  const Tc32Share s = tc32_share(p, e, wg);
+  const uint32_t b_base = rg.b_base + (uint32_t)s.c_off * 64u;     // 64-byte weight rows
   const uint32_t box = rg.e_base + (uint32_t)wg * (64u * N * 4u), bias_s = rg.bias_base + (uint32_t)wg * (N * 4u);
   const uint32_t rbar = rg.rfull(wg);
   uint32_t rphase = 0;
@@ -376,14 +394,14 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
   const uint32_t a_pitch = halo ? (uint32_t)p.halo_w * 64u : 512u;      // byte distance of the A planes' 8-row groups
   const uint64_t a_hi = desc_hi(64u, a_pitch), b_hi = desc_hi(64u, 512u);
   // this warpgroup's 64 pixels: row0 / 8 halo rows (of 8 tile pixels each) down, or row0 dense rows
-  const uint32_t a_wg = halo ? (uint32_t)(row0 >> 3) * a_pitch : (uint32_t)row0 * 64u;
+  const uint32_t a_wg = halo ? (uint32_t)(s.row0 >> 3) * a_pitch : (uint32_t)s.row0 * 64u;
   const uint32_t plane = (uint32_t)e.plane_bytes, b_plane = (uint32_t)e.b_plane_bytes;
   float acc[N / 2], sum[N / 2];
   RingPos ap, bp;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     float bias_v = 0.f;
     if (epi_tma) {        // this thread's bias value of the tile: loaded now, written to shared memory in the epilogue
-      const int c = tile_coord(p, tile).n_idx * N + (threadIdx.x & 127);
+      const int c = tile_coord(p, tile).n_idx * p.block_n + tc32_share(p, e, wg).c_off + (threadIdx.x & 127);
       if (p.bias && (threadIdx.x & 127) < N && c < p.cout) bias_v = __ldg(p.bias + c);
     }
 #pragma unroll
@@ -398,7 +416,7 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
         }
         bp.wait_full(rg.bfull(bp.slot));
         const uint32_t a_addr = halo ? a_item + (uint32_t)tap.r * a_pitch + (uint32_t)tap.s * 64u : a_item;
-        const uint32_t b_addr = rg.b_base + bp.slot * rg.b_bytes + b_off;
+        const uint32_t b_addr = b_base + bp.slot * rg.b_bytes;
         const uint64_t A = desc_at(a_hi, a_addr), A2 = desc_at(a_hi, a_addr + plane);
         const uint64_t B = desc_at(b_hi, b_addr), B2 = desc_at(b_hi, b_addr + b_plane);
         wg::fence();
@@ -425,7 +443,7 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
           if (item_done) mbar_arrive(rg.pempty(ap.slot));
           if (epi_tma && p.res && cc == 0 && tap.k == 0) {
             asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-            const EpiBox eb = epi_box(p, tile, wg);
+            const EpiBox eb = epi_box(p, e, tile, wg);
             if (eb.live) {
               mbar_expect_tx(rbar, 64u * N * 4u);
 #pragma unroll
@@ -441,10 +459,11 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
       }
     }
     if (epi_tma) {
-      epi_tma32<N>(p, tmY, sum, box, bias_s, bias_v, rbar, rphase, wg, tile);
+      epi_tma32<N>(p, e, tmY, sum, box, bias_s, bias_v, rbar, rphase, wg, tile);
       if (p.res) rphase ^= 1u;
     } else {
-      epi_frag<N, 4>(p, sum, tile, row0, c_off);
+      const Tc32Share s = tc32_share(p, e, wg);
+      epi_frag<N, 4>(p, sum, tile, s.row0, s.c_off);
     }
   }
   // the boxes must stay allocated until the last store has read them, and the stores must be complete before the grid is
@@ -455,13 +474,13 @@ __device__ __forceinline__ void consumer32(const ConvTcParams& p, const Tc32Extr
 template <int NWG, bool TMA_EPI>
 __device__ __forceinline__ void consumer32_n(const ConvTcParams& p, const Tc32Extra& e, const Ring32& rg, int wg,
                                              const CUtensorMap* tmY, const CUtensorMap* tmR) {
-  switch (p.block_n) {
-    case 16: consumer32<16, TMA_EPI>(p, e, rg, wg, 64 * wg, 0u, 0, tmY, tmR); break;
-    case 32: consumer32<32, TMA_EPI>(p, e, rg, wg, 64 * wg, 0u, 0, tmY, tmR); break;
-    case 64: consumer32<64, TMA_EPI>(p, e, rg, wg, 64 * wg, 0u, 0, tmY, tmR); break;
+  switch (p.block_n / e.wg_n) {
+    case 16: consumer32<16, TMA_EPI>(p, e, rg, wg, tmY, tmR); break;
+    case 32: consumer32<32, TMA_EPI>(p, e, rg, wg, tmY, tmR); break;
+    case 64: consumer32<64, TMA_EPI>(p, e, rg, wg, tmY, tmR); break;
     default:
-      if constexpr (NWG == 2 && !TMA_EPI) consumer32<T32_MAX_N, false>(p, e, rg, wg, 64 * wg, 0u, 0, tmY, tmR);
-      else __trap();                      // the host plan pairs block_n > T32_EPI_MAX_N with neither NWG = 4 nor the TMA epilogue
+      if constexpr (NWG == 2 && !TMA_EPI) consumer32<T32_MAX_N, false>(p, e, rg, wg, tmY, tmR);
+      else __trap();                      // the host plan pairs N > T32_EPI_MAX_N with neither NWG = 4 nor the TMA epilogue
       break;
   }
 }
@@ -519,14 +538,11 @@ dcn_igemm_tc32_kernel(const __grid_constant__ CUtensorMap tmB, const ConvTcParam
   if (warp >= 4 && warp < 12) {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(DCN32_HI_REGS));
     const int wg = (warp - 4) >> 2;
-    const int bn = e.dcn_split_n ? p.block_n / 2 : p.block_n;
-    const int row0 = e.dcn_split_n ? 0 : 64 * wg, c_off = e.dcn_split_n ? bn * wg : 0;
-    const uint32_t b_off = (uint32_t)c_off * 64u;       // 64-byte weight rows
-    switch (bn) {
-      case 16: consumer32<16, false>(p, e, rg, wg, row0, b_off, c_off, nullptr, nullptr); break;
-      case 32: consumer32<32, false>(p, e, rg, wg, row0, b_off, c_off, nullptr, nullptr); break;
-      case 64: consumer32<64, false>(p, e, rg, wg, row0, b_off, c_off, nullptr, nullptr); break;
-      default: consumer32<DCN32_MAX_N, false>(p, e, rg, wg, row0, b_off, c_off, nullptr, nullptr); break;
+    switch (p.block_n / e.wg_n) {
+      case 16: consumer32<16, false>(p, e, rg, wg, nullptr, nullptr); break;
+      case 32: consumer32<32, false>(p, e, rg, wg, nullptr, nullptr); break;
+      case 64: consumer32<64, false>(p, e, rg, wg, nullptr, nullptr); break;
+      default: consumer32<DCN32_MAX_N, false>(p, e, rg, wg, nullptr, nullptr); break;
     }
   } else {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(DCN32_LO_REGS));
@@ -583,7 +599,7 @@ constexpr int T32_SMEM_MAX = 227 * 1024 - 64;    // dynamic shared memory of a t
 struct Tc32Plan {
   ConvTcParams p;
   Tc32Extra e;
-  int nwg;                   // convolution: consumer warpgroups, the tile holds 64 * nwg output pixels
+  int nwg;                   // convolution: consumer warpgroups, the tile holds 64 * nwg / e.wg_n output pixels
   int epi_tma;               // 1: TMA epilogue (output boxes in shared memory), 0: stores from the accumulator fragments
   int smem;                  // dynamic shared memory
 };
@@ -600,12 +616,14 @@ bool tc32_epi_expressible(const vps_conv_args* a, int nprob) {
   return true;
 }
 
-// The tile of nwg consumer warpgroups x block_n channels and its A items; tc32_plan sets the weight ring depth.
-Tc32Plan tc32_tile(const vps_conv_args* a, int nprob, int nwg, int block_n) {
+// The tile of nwg consumer warpgroups in layout (nwg / wg_n, wg_n), n channels each, and its A items; tc32_plan sets the
+// weight ring depth.
+Tc32Plan tc32_tile(const vps_conv_args* a, int nprob, int nwg, int wg_n, int n) {
   Tc32Plan g = {};
   ConvTcParams& p = g.p;
   g.nwg = nwg;
-  const int px = 64 * nwg;
+  g.e.wg_n = wg_n;
+  const int px = 64 * (nwg / wg_n), block_n = wg_n * n;
   p.halo = a->sh == 1 && a->sw == 1 && a->kh * a->kw > 1 && a->kh <= 8 && a->kw <= 8;
   // 8-pixel halo rows: the consumer's descriptors step one halo row per 8-row group
   const int tw = p.halo ? 8 : patch_tw(a->oh, a->ow, px, a->sh, a->sw);
@@ -620,17 +638,21 @@ Tc32Plan tc32_tile(const vps_conv_args* a, int nprob, int nwg, int block_n) {
   return g;
 }
 
-// (NWG, block_n) minimising waves * (steps * step clocks + epilogue) over the candidates whose rings fit (>= 2 weight
-// stages).  block_n is a power-of-two divisor of cout_pad, <= 128 at NWG 2 and <= 64 at NWG 4 (the register cap).
-// A step of one warpgroup is two dependent wgmma round trips plus its barrier waits: ~300 clocks whatever N is (the latency
-// floor); its 6 MMAs take 3*bn clocks of the tensor pipe per 2 warpgroups, so 6*bn at NWG 4; its weight tile arrives at
-// the L2 rate (56 B/clk per SM); and the three converter warps turn an A item of `rows` pixels into operand planes at ~2
-// clocks per row -- in flat mode every step is a new item (256 rows at NWG 4), in halo mode one item feeds all taps.
-// So NWG 4 shares the latency floor among twice the pixels and halves the per-tile epilogue, and wins wherever the grid
-// has enough tiles; it loses where the converters bind: flat layers with many K steps whose cout_pad > 64 must be split
-// into more N tiles at NWG 4, each converting the same activations again (3x3 / stride 2, 128 -> 128 at 256x512 ran 15%
-// slower).  The 2 clocks per row is the value that keeps those on NWG 2 and every layer that measured faster on NWG 4;
-// per-layer H100 timings are in DESIGN.md §5.0.
+// (NWG, Q, N) minimising waves * (steps * step clocks + epilogue) over the candidates whose rings fit (>= 2 weight
+// stages).  N (channels per warpgroup) is <= 128 at NWG 2 and <= 64 at NWG 4 (the register cap), and block_n = Q N is a
+// power-of-two divisor of cout_pad.  The layouts: NWG 2 as (2, 1); NWG 4 as (4, 1), and as (2, 2) and (1, 4) at N = 64.
+// Channel groups of fewer than 64 channels, and (1, 2) at NWG 2, never measured faster than a (P, 1) layout on the
+// production shapes, so they are not candidates.  The step costs are fitted to H100 per-layer times of every candidate on
+// the shapes of tools/diag_tc32.py (DESIGN.md §5.0) and add up rather than overlap:
+//   * a fixed 410 clocks (the two dependent wgmma round trips, barrier waits), 70 more at 640 threads;
+//   * the tensor pipe: 6 NWG MMAs of m64 x N x k16 at 2048 MAC/clk = 3 NWG N clocks; at NWG 2, 0.4 N more (one warpgroup's
+//     longer MMA chain is hidden only by the other);
+//   * the converters: 6 clocks per activation row they convert (an A item per step in flat mode, per channel chunk in halo
+//     mode), so a tile that spans more channels converts each input row for more of them;
+//   * the weight tile: 1 clock per 200 bytes of it.
+// The epilogue costs 40 N + 1500 clocks per tile.  A shared-memory read term (every MMA reading its A and B slabs at
+// 128 B/clk) did not fit the timings: (1, 4), which reads the most, is the fastest layout wherever it fits.
+constexpr double T32_STEP_CLK = 410.0, T32_STEP_CLK_640 = 70.0, T32_MMA_CLK_N2 = 0.4, T32_CONV_CLK = 6.0, T32_B_BYTES_PER_CLK = 200.0;
 int tc32_plan(const vps_conv_args* a, int nprob, Tc32Plan& out) {
   VPS_CHECK_ARG(nprob >= 1 && nprob <= MAX_PROB, "conv2d_tc32: nprob %d", nprob);
   VPS_CHECK_ARG(a->sh >= 1 && a->sh <= 2 && a->sw >= 1 && a->sw <= 2, "conv2d_tc32: stride must be 1 or 2");
@@ -640,20 +662,24 @@ int tc32_plan(const vps_conv_args* a, int nprob, Tc32Plan& out) {
   if (sms <= 0) { vps::set_error("no device"); return VPS_E_NODEV; }
   const int cout_pad = (a->cout + 15) / 16 * 16;
   double best = -1.0;
-  for (int nwg = 2; nwg <= 4; nwg += 2) {
-    for (int bn = 16; bn <= (nwg == 2 ? T32_MAX_N : T32_WIDE_MAX_N) && bn <= cout_pad; bn *= 2) {
-      if (cout_pad % bn) continue;
-      Tc32Plan g = tc32_tile(a, nprob, nwg, bn);
-      g.p.b_stages = 2;
-      if ((int)ring32(0, g.p, g.e, nwg, false, false).smem > T32_SMEM_MAX) continue;
-      const int64_t tiles = g.p.total_tiles;
-      const double waves = (double)((tiles + sms - 1) / sms);
-      const double conv = 2.0 * (g.p.halo ? (double)g.e.rows / (a->kh * a->kw) : (double)g.e.rows);
-      const double step = fmax(fmax(300.0, 1.5 * nwg * bn), fmax((double)(bn * 64 * T32_PLANES) / 56.0, conv));
-      const double t = waves * ((double)tc32_walk(g.p).steps() * step + 40.0 * bn + 1500.0);
-      if (best < 0 || t < best * 0.999) {
-        best = t;
-        out = g;
+  for (int wg_n = 1; wg_n <= 4; wg_n *= 2) {
+    for (int nwg = 2; nwg <= 4; nwg += 2) {
+      if (wg_n > 1 && nwg == 2) continue;
+      for (int n = 16; n <= (nwg == 2 ? T32_MAX_N : T32_WIDE_MAX_N) && wg_n * n <= cout_pad; n *= 2) {
+        if (cout_pad % (wg_n * n) || (wg_n > 1 && n != T32_WIDE_MAX_N)) continue;
+        Tc32Plan g = tc32_tile(a, nprob, nwg, wg_n, n);
+        g.p.b_stages = 2;
+        if ((int)ring32(0, g.p, g.e, nwg, false, false).smem > T32_SMEM_MAX) continue;
+        const int64_t tiles = g.p.total_tiles;
+        const double waves = (double)((tiles + sms - 1) / sms);
+        const double rows = g.p.halo ? (double)g.e.rows / (a->kh * a->kw) : (double)g.e.rows;
+        const double step = T32_STEP_CLK + (nwg == 4 ? T32_STEP_CLK_640 : T32_MMA_CLK_N2 * n) + 3.0 * nwg * n + T32_CONV_CLK * rows +
+                            (double)(g.p.block_n * 64 * T32_PLANES) / T32_B_BYTES_PER_CLK;
+        const double t = waves * ((double)tc32_walk(g.p).steps() * step + 40.0 * n + 1500.0);
+        if (best < 0 || t < best * 0.999) {
+          best = t;
+          out = g;
+        }
       }
     }
   }
@@ -669,7 +695,7 @@ int tc32_plan(const vps_conv_args* a, int nprob, Tc32Plan& out) {
   ConvTcParams& p = out.p;
   p.b_stages = 2;
   const auto epi_fits = [&] { return (int)ring32(0, p, out.e, out.nwg, true, false).smem <= T32_SMEM_MAX; };
-  if (!p.halo && p.block_n <= T32_EPI_MAX_N && tc32_epi_expressible(a, nprob)) {
+  if (!p.halo && p.block_n / out.e.wg_n <= T32_EPI_MAX_N && tc32_epi_expressible(a, nprob)) {
     if (!epi_fits() && p.a_stages == 3) {
       p.a_stages = 2;
       if (!epi_fits()) p.a_stages = 3;
@@ -689,7 +715,7 @@ int tc32_plan(const vps_conv_args* a, int nprob, Tc32Plan& out) {
 constexpr int DCN32_SMEM_MAX = 132 * 1024;
 // Clocks of the CTA's 7 sampling warps per 8-pixel x 32-channel unit, from per-layer H100 timings of the 128-pixel x 64
 // tiling (DESIGN.md §5.0: about 120 ns at every layer and level; the units are latency bound, 7 in flight per CTA), and the
-// latency floor of a consumer K step (two dependent wgmma round trips, as in tc32_plan).
+// latency floor of a consumer K step (two dependent wgmma round trips).
 constexpr double DCN32_UNIT_CLK = 220.0, DCN32_STEP_CLK = 300.0;
 
 // (layout, bn) minimising waves * (K steps * step clocks + epilogue), among those whose tile width divides cout_pad and whose
@@ -711,7 +737,7 @@ int dcn32_plan(const vps_conv_args* a, Tc32Plan& out) {
       Tc32Plan g = {};
       set_tiles(g.p, a, 1, tw, rows / tw, block_n, T32_KC);
       g.p.a_stages = 2;
-      g.e.rows = rows; g.e.plane_bytes = rows * 64; g.e.b_plane_bytes = block_n * 64; g.e.dcn = 1; g.e.dcn_split_n = split_n;
+      g.e.rows = rows; g.e.plane_bytes = rows * 64; g.e.b_plane_bytes = block_n * 64; g.e.dcn = 1; g.e.wg_n = split_n ? 2 : 1;
       const Ring32 rg = ring32(0, g.p, g.e, 2, false, true);
       const int bst = (DCN32_SMEM_MAX - (int)rg.smem) / (int)rg.b_bytes;
       if (bst < 2) continue;
@@ -809,7 +835,7 @@ extern "C" int vps_conv2d_tc32_multi(const vps_conv_args* args, int nprob, void*
   // keeps its pixel stride); TMA clips the boxes at oh / ow / cout, so partial tiles and the neighbouring channels are safe
   CUtensorMap tmY = {}, tmR = {};
   if (g.epi_tma) {
-    const int bc = t32_box_c(p.block_n), box_w = p.tw < 64 ? p.tw : 64;
+    const int bc = t32_box_c(p.block_n / g.e.wg_n), box_w = p.tw < 64 ? p.tw : 64;
     const int64_t px = (int64_t)a->oy_off * a->y.w + a->ox_off;
     for (int m = 0; m < (a->res.ptr ? 2 : 1); ++m) {
       const vps_tensor& t = m ? a->res : a->y;          // the residual has the output's geometry
@@ -836,6 +862,7 @@ extern "C" int vps_conv2d_tc32_plan(const vps_conv_args* a, int nprob, int* plan
   const int st = tc32_plan(a, nprob, g);
   if (st != VPS_OK) return st;
   plan[0] = g.nwg; plan[1] = g.p.block_n; plan[2] = g.p.tw; plan[3] = g.p.th; plan[4] = g.p.halo; plan[5] = g.epi_tma;
+  plan[6] = g.e.wg_n;
   return VPS_OK;
 }
 
@@ -881,6 +908,6 @@ extern "C" int vps_deform_conv_tc32_plan(const vps_tensor* x, int cout, int* pla
   Tc32Plan g;
   const int st = dcn32_plan(&a, g);
   if (st != VPS_OK) return st;
-  plan[0] = g.e.rows; plan[1] = g.e.dcn_split_n ? g.p.block_n / 2 : g.p.block_n; plan[2] = g.e.dcn_split_n; plan[3] = g.p.n_tiles_n;
+  plan[0] = g.e.rows; plan[1] = g.p.block_n / g.e.wg_n; plan[2] = g.e.wg_n == 2; plan[3] = g.p.n_tiles_n;
   return VPS_OK;
 }

@@ -271,17 +271,19 @@ def conv2d_tc_multi(x, pws, y, pads, omaps, act=ACT_NONE, slope=0.1, out_scale=1
 def conv2d_tc32_plan(x, pws, stride=1, pad=0, oh=None, ow=None, pads=None, y=None, res=None, omaps=None):
     """The tiling the tc32 kernel picks for conv2d (one problem) or conv2d_tc_multi (`pads` = per-phase (ph, pw), stride 1,
     `omaps` = per-phase output maps) writing into `y` (default: x) with residual `res`: dict(nwg=consumer warpgroups (2 or 4),
-    block_n, tw, th (output pixels per tile), halo, epilogue="tma" (output boxes in shared memory, TMA store) or "frag"
-    (stores from the accumulator fragments))."""
+    block_n (channels per tile), tw, th (output pixels per tile), halo, epilogue="tma" (output boxes in shared memory, TMA
+    store) or "frag" (stores from the accumulator fragments), wg_n=Q (channel groups: each warpgroup takes block_n / Q
+    channels of 64 pixels), layout=(P, Q) with P * Q = nwg)."""
     pws = pws if isinstance(pws, (list, tuple)) else [pws]
     n = len(pws)
     arr = (VpsConvArgs * n)()
     for i in range(n):
         arr[i] = _conv_args(x, pws[i], x if y is None else y, stride, pad, ACT_NONE, 0.1, res, False, 1.0, oh, ow,
                             omaps[i] if omaps is not None else (1, 0, 1, 0), pads[i] if pads is not None else None)
-    plan = (C.c_int * 6)()
+    plan = (C.c_int * 7)()
     check(_real_lib().vps_conv2d_tc32_plan(arr, n, plan), "conv2d_tc32_plan")
-    return dict(nwg=plan[0], block_n=plan[1], tw=plan[2], th=plan[3], halo=plan[4], epilogue="tma" if plan[5] else "frag")
+    return dict(nwg=plan[0], block_n=plan[1], tw=plan[2], th=plan[3], halo=plan[4], epilogue="tma" if plan[5] else "frag",
+                wg_n=plan[6], layout=(plan[0] // plan[6], plan[6]))
 
 
 def conv2d_tc_plan(x, pws, stride=1, pad=0, oh=None, ow=None, pads=None, y=None, res=None, omaps=None):

@@ -63,6 +63,11 @@ def init_weights(model, kind="C", seed=0):
                 m.weight.fill_(1); m.bias.zero_(); m.running_mean.zero_(); m.running_var.fill_(1)
                 if name.endswith("bn3"):
                     m.weight.zero_()
+            elif m.__class__.__name__ in ("DeformConv", "_DeformConv"):
+                # the reference's DeformConv.reset_parameters (uniform +-1/sqrt(fan_in)), drawn from the seeded generator:
+                # left to the constructor, these weights came from the global RNG and changed with whatever ran before
+                stdv = 1.0 / math.sqrt(m.weight[0].numel())
+                U(m.weight, -stdv, stdv)
         return model
 
     for name, m in model.named_modules():
