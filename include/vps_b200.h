@@ -304,7 +304,11 @@ int vps_maskroi_candidates(const float* rois, const float* cls_score, const floa
  * comp = log_softmax([0|dots]) + c0*log(p) + c1*[0|IoU] + c2*[1|label eq], row argmax (first max),
  * then the sequential id-assignment loop on one device thread.  Outputs det_obj_ids[k], match_ids[k],
  * comp_scores [k,m+1], mem_src[cap] (detection whose RoI features/box end in memory slot j, -1 =
- * unchanged) and *new_m.  ws >= (k*m + k + 2*cap)*4 bytes. */
+ * unchanged) and *new_m <= m + k.  ws >= (k*m + k + 2*cap)*4 bytes; the dots stay in ws[0, k*m) (floats,
+ * row-major [k,m]).  Each dot is lane 0's value of one warp that runs an fmaf chain per column class
+ * c = lane (mod 32), in increasing c, followed by the xor butterfly over o = 16..1.  The memory is the caller's
+ * and has no size limit here: the caller grows it so that m + k <= cap (a detection appends at most one slot);
+ * `cap` only sizes mem_src and ws. */
 int vps_track_assign(const float* emb, const float* ref_emb, int k, int m, int dim, const float* det_boxes,
                      const float* ref_boxes, const int32_t* det_labels, const int32_t* ref_labels,
                      const float* cls_prob, float c0, float c1, float c2, int cap, int32_t* det_obj_ids,
@@ -331,7 +335,10 @@ int vps_det_split(const float* det_rois, const int32_t* cls_idx, int cap, float*
 /* mask_score.gather(1, cls_idx) (panoptic_fusetrack.py:566-568): logits NHWC [>=k,ms,ms,9] -> out f32 [k,ms,ms] */
 int vps_select_class(const vps_tensor* logits, const int32_t* cls_idx, int k, float* out, void* stream);
 /* tracker memory update (panoptic_fusetrack.py:441-443,458-459,467-469): for j < *new_m with mem_src[j] >= 0:
- * mem_feats[j] <- det_feats[mem_src[j]], mem_boxes likewise, mem_labels only for appended slots (j >= old_m). */
+ * mem_feats[j] <- det_feats[mem_src[j]] (rows of feat_len elements of `dtype`), mem_boxes likewise, mem_labels only for
+ * appended slots (j >= old_m).  mem_boxes / det_boxes and mem_labels / det_labels may be NULL: the same row scatter then
+ * updates any per-slot table, e.g. the cached fp32 track embeddings.  Reads mem_src[0, *new_m) once and copies only the
+ * written rows; any cap (> 0) is accepted. */
 int vps_track_update(void* mem_feats, const void* det_feats, int dtype, int64_t feat_len, float* mem_boxes,
                      const float* det_boxes, int32_t* mem_labels, const int32_t* det_labels,
                      const int32_t* mem_src, int old_m, int cap, const int* new_m_dev, void* stream);

@@ -269,20 +269,108 @@ __global__ void maskroi_candidates_kernel(const float* __restrict__ rois, const 
 }
 
 // ------------------------------------------------------------------ tracker
-// dots[i][j] = <emb_i, ref_j>, one warp per pair
-__global__ void track_dot_kernel(const float* __restrict__ emb, const float* __restrict__ ref, int k, int m, int dim,
-                                 float* __restrict__ dots) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
-  const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  for (int64_t pr = warp; pr < (int64_t)k * m; pr += nw) {
-    const int i = (int)(pr / m), j = (int)(pr % m);
-    const float* a = emb + (int64_t)i * dim;
-    const float* b = ref + (int64_t)j * dim;
-    float s = 0.f;
-    for (int c = lane; c < dim; c += 32) s = fmaf(a[c], b[c], s);
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) dots[pr] = s;
+// dots[i][j] = <emb_i, ref_j>.  The bits are those of one warp per pair: lane l runs an fmaf chain from 0 over the columns
+// c = l (mod 32) in increasing c, then the xor butterfly s += shfl_xor(s, o) for o = 16, 8, 4, 2, 1 (lane 0's value; the
+// comp scores of the tracker, and so its ids, depend on these bits).
+//
+// Tiling: a block owns TD_BI detections x TD_BJ memory slots (blockIdx.x = slot tile * detection tiles + detection tile,
+// so the blocks that read the same memory rows run together and each row comes from DRAM about once), stages the rows
+// through shared memory TD_CK columns at a time (cp.async, double-buffered), and each warp keeps a TD_TI x TD_TJ
+// register tile of pairs: lane l holds the partial sums of column class l of all 64 pairs.  The butterfly then runs as
+// a reduce-scatter: step o exchanges half of the sums a lane holds with lane l ^ o and adds, so every pair goes through
+// the same additions as above (IEEE addition commutes), and lane l ends with pairs 2l and 2l + 1.
+constexpr int TD_TI = 8, TD_TJ = 8;              // register tile of a warp: detections x slots
+constexpr int TD_WI = 2, TD_WJ = 4;              // warps of a block: detections x slots
+constexpr int TD_BI = TD_TI * TD_WI, TD_BJ = TD_TJ * TD_WJ, TD_CK = 128, TD_THREADS = 32 * TD_WI * TD_WJ;
+static_assert((TD_BI + TD_BJ) * TD_CK % TD_THREADS == 0 && 2 * (TD_BI + TD_BJ) * TD_CK * 4 <= 48 * 1024, "staging");
+static_assert(TD_TI * TD_TJ == 64, "the reduce-scatter below leaves 2 of 64 pairs per lane");
+
+// one butterfly step over the first H sums of v: keep one half (by lane bit O), add the partner's sums of that half
+template <int O, int H>
+__device__ __forceinline__ void dot_scatter_step(float (&v)[TD_TI * TD_TJ], int lane) {
+  const bool up = (lane & O) != 0;
+#pragma unroll
+  for (int r = 0; r < H / 2; ++r) {
+    const float send = up ? v[r] : v[r + H / 2];
+    const float keep = up ? v[r + H / 2] : v[r];
+    v[r] = keep + __shfl_xor_sync(0xffffffffu, send, O);
+  }
+}
+
+// 4-byte asynchronous global -> shared copy; src_bytes 0 stores a zero (rows past k / m, columns past dim)
+__device__ __forceinline__ void cp_async4(float* dst, const float* src, int src_bytes) {
+  const unsigned d = (unsigned)__cvta_generic_to_shared(dst);
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(d), "l"(src), "r"(src_bytes) : "memory");
+}
+
+__global__ void __launch_bounds__(TD_THREADS, 2)
+track_dot_kernel(const float* __restrict__ emb, const float* __restrict__ ref, int k, int m, int dim,
+                 float* __restrict__ dots) {
+  // two stages of TD_CK columns: detection rows [0, TD_BI), memory rows [TD_BI, TD_BI + TD_BJ); the copy of the next
+  // chunk runs while the warps multiply the current one
+  __shared__ float st[2][TD_BI + TD_BJ][TD_CK];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int wi = warp / TD_WJ, wj = warp % TD_WJ;
+  const int ntile_i = (k + TD_BI - 1) / TD_BI;
+  const int i0 = (int)(blockIdx.x % ntile_i) * TD_BI;
+  const int64_t j0 = (int64_t)(blockIdx.x / ntile_i) * TD_BJ;
+  auto stage = [&](int buf, int c0) {
+#pragma unroll 1
+    for (int it = 0; it < (TD_BI + TD_BJ) * TD_CK / TD_THREADS; ++it) {
+      const int e = it * TD_THREADS + threadIdx.x;
+      const int r = e / TD_CK, c = e % TD_CK;
+      const float* src = emb;
+      bool ok = c0 + c < dim;
+      if (r < TD_BI) {
+        ok = ok && i0 + r < k;
+        if (ok) src = emb + (int64_t)(i0 + r) * dim + c0 + c;
+      } else {
+        const int64_t j = j0 + r - TD_BI;
+        ok = ok && j < m;
+        if (ok) src = ref + j * dim + c0 + c;
+      }
+      // a staged zero leaves the chain unchanged: fmaf(0, 0, s) == s for every s the chain can hold (never -0)
+      cp_async4(&st[buf][r][c], src, ok ? 4 : 0);
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  float acc[TD_TI * TD_TJ];
+#pragma unroll
+  for (int q = 0; q < TD_TI * TD_TJ; ++q) acc[q] = 0.f;
+  stage(0, 0);
+  for (int c0 = 0, buf = 0; c0 < dim; c0 += TD_CK, buf ^= 1) {
+    if (c0 + TD_CK < dim) {
+      stage(buf ^ 1, c0 + TD_CK);
+      asm volatile("cp.async.wait_group 1;" ::: "memory");
+    } else {
+      asm volatile("cp.async.wait_group 0;" ::: "memory");
+    }
+    __syncthreads();                                   // chunk c0 is in st[buf] for every thread
+#pragma unroll
+    for (int t = 0; t < TD_CK / 32; ++t) {           // columns c0 + 32 t + lane: increasing c per lane
+      float a[TD_TI], b[TD_TJ];
+#pragma unroll
+      for (int ti = 0; ti < TD_TI; ++ti) a[ti] = st[buf][wi * TD_TI + ti][t * 32 + lane];
+#pragma unroll
+      for (int tj = 0; tj < TD_TJ; ++tj) b[tj] = st[buf][TD_BI + wj * TD_TJ + tj][t * 32 + lane];
+#pragma unroll
+      for (int ti = 0; ti < TD_TI; ++ti)
+#pragma unroll
+        for (int tj = 0; tj < TD_TJ; ++tj) acc[ti * TD_TJ + tj] = fmaf(a[ti], b[tj], acc[ti * TD_TJ + tj]);
+    }
+    __syncthreads();                                   // st[buf] is read before the copy two chunks on refills it
+  }
+  dot_scatter_step<16, 64>(acc, lane);
+  dot_scatter_step<8, 32>(acc, lane);
+  dot_scatter_step<4, 16>(acc, lane);
+  dot_scatter_step<2, 8>(acc, lane);
+  dot_scatter_step<1, 4>(acc, lane);
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int q = 2 * lane + r;
+    const int i = i0 + wi * TD_TI + q / TD_TJ;
+    const int64_t j = j0 + wj * TD_TJ + q % TD_TJ;
+    if (i < k && j < m) dots[(int64_t)i * m + j] = acc[r];
   }
 }
 
@@ -334,15 +422,22 @@ __global__ void track_score_kernel(const float* __restrict__ dots, int k, int m,
   if (lane == 0) { match_ids[i] = besti; match_like[i] = best; }
 }
 
-// the sequential id-assignment loop (panoptic_fusetrack.py:430-469) on one thread.
+// state of the id-assignment loop: no slot written, no best match per memory slot yet
+__global__ void track_assign_init_kernel(int m, int cap, int32_t* __restrict__ mem_src, float* __restrict__ best_scores,
+                                         int32_t* __restrict__ best_ids) {
+  VPS_GRID_STRIDE(j, cap) {
+    mem_src[j] = -1;
+    if (j < m) { best_scores[j] = -100.f; best_ids[j] = -1; }
+  }
+}
+
+// the sequential id-assignment loop (panoptic_fusetrack.py:430-469) on one thread, O(k).
 // mem_src[slot] = index of the detection whose features/box end up in memory slot `slot` (-1: unchanged).
 __global__ void track_assign_kernel(const int32_t* __restrict__ match_ids, const float* __restrict__ match_like, int k,
                                     int m, int cap, int32_t* __restrict__ det_obj_ids, int32_t* __restrict__ mem_src,
                                     float* __restrict__ best_scores, int32_t* __restrict__ best_ids, int* __restrict__ new_m) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   int cur = m;
-  for (int j = 0; j < cap; ++j) mem_src[j] = -1;
-  for (int j = 0; j < m; ++j) { best_scores[j] = -100.f; best_ids[j] = -1; }
   for (int i = 0; i < k; ++i) det_obj_ids[i] = -1;
   for (int i = 0; i < k; ++i) {
     const int mid = match_ids[i];
@@ -446,20 +541,40 @@ __global__ void select_class_kernel(vps::TV<const T> logits, const int32_t* __re
   }
 }
 
-// tracker memory update (panoptic_fusetrack.py:441-443,458-459,467-469): slot j <- detection mem_src[j]
+// tracker memory update (panoptic_fusetrack.py:441-443,458-459,467-469): slot j <- detection mem_src[j].
+// Block b owns the slots j = b (mod gridDim.x): it reads their mem_src entries TU_THREADS at a time, lists the written
+// ones in shared memory and copies each listed row with all its threads, so the work is one scan of mem_src[0, new_m)
+// plus the written rows, and consecutive written slots (the appended ones) go to different blocks.
+constexpr int TU_THREADS = 256, TU_BLOCKS = 512;
 template <typename T>
-__global__ void track_update_kernel(T* __restrict__ mem_feats, const T* __restrict__ det_feats, int64_t feat_len,
-                                    float* __restrict__ mem_boxes, const float* __restrict__ det_boxes,
-                                    int32_t* __restrict__ mem_labels, const int32_t* __restrict__ det_labels,
-                                    const int32_t* __restrict__ mem_src, int old_m, const int* __restrict__ new_m_dev) {
-  const int j = blockIdx.y;
-  if (j >= *new_m_dev) return;
-  const int src = mem_src[j];
-  if (src < 0) return;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < feat_len; i += (int64_t)gridDim.x * blockDim.x)
-    mem_feats[(int64_t)j * feat_len + i] = det_feats[(int64_t)src * feat_len + i];
-  if (blockIdx.x == 0 && threadIdx.x < 4) mem_boxes[(int64_t)j * 4 + threadIdx.x] = det_boxes[(int64_t)src * 4 + threadIdx.x];
-  if (blockIdx.x == 0 && threadIdx.x == 0 && j >= old_m) mem_labels[j] = det_labels[src];
+__global__ void __launch_bounds__(TU_THREADS)
+track_update_kernel(T* __restrict__ mem_feats, const T* __restrict__ det_feats, int64_t feat_len,
+                    float* __restrict__ mem_boxes, const float* __restrict__ det_boxes, int32_t* __restrict__ mem_labels,
+                    const int32_t* __restrict__ det_labels, const int32_t* __restrict__ mem_src, int old_m,
+                    const int* __restrict__ new_m_dev) {
+  __shared__ int64_t slot[TU_THREADS];
+  __shared__ int src[TU_THREADS];
+  __shared__ int nlist;
+  const int64_t n = *new_m_dev;
+  for (int64_t s0 = 0; blockIdx.x + s0 * gridDim.x < n; s0 += TU_THREADS) {
+    if (threadIdx.x == 0) nlist = 0;
+    __syncthreads();
+    const int64_t j = blockIdx.x + (s0 + threadIdx.x) * gridDim.x;
+    const int s = j < n ? mem_src[j] : -1;
+    if (s >= 0) {
+      const int p = atomicAdd(&nlist, 1);
+      slot[p] = j;
+      src[p] = s;
+    }
+    __syncthreads();
+    for (int q = 0; q < nlist; ++q) {
+      const int64_t jj = slot[q], ss = src[q];
+      for (int64_t i = threadIdx.x; i < feat_len; i += TU_THREADS) mem_feats[jj * feat_len + i] = det_feats[ss * feat_len + i];
+      if (mem_boxes != nullptr && threadIdx.x < 4) mem_boxes[jj * 4 + threadIdx.x] = det_boxes[ss * 4 + threadIdx.x];
+      if (mem_labels != nullptr && threadIdx.x == 0 && jj >= old_m) mem_labels[jj] = det_labels[ss];
+    }
+    __syncthreads();                                   // the list is read before the next round resets it
+  }
 }
 
 
@@ -589,8 +704,12 @@ extern "C" int vps_track_assign(const float* emb, const float* ref_emb, int k, i
   float* match_like = dots + (int64_t)k * m;
   float* best_scores = match_like + k;
   int32_t* best_ids = (int32_t*)(best_scores + cap);
-  track_dot_kernel<<<vps::grid_for((int64_t)k * m * 32), 256, 0, st>>>(emb, ref_emb, k, m, dim, dots);
+  const int64_t dot_blocks = (int64_t)vps::cdiv(k, TD_BI) * vps::cdiv(m, TD_BJ);
+  VPS_CHECK_ARG(dot_blocks <= 0x7fffffff, "track_assign: k %d x m %d exceeds one grid", k, m);
+  track_dot_kernel<<<(unsigned)dot_blocks, TD_THREADS, 0, st>>>(emb, ref_emb, k, m, dim, dots);
   VPS_CUDA_LAST("track_dot");
+  track_assign_init_kernel<<<vps::grid_for(cap), 256, 0, st>>>(m, cap, mem_src, best_scores, best_ids);
+  VPS_CUDA_LAST("track_assign_init");
   track_score_kernel<<<vps::cdiv((int64_t)k * 32, 128), 128, 0, st>>>(dots, k, m, det_boxes, ref_boxes, det_labels,
                                                                      ref_labels, cls_prob, c0, c1, c2, comp_scores,
                                                                      match_ids, match_like);
@@ -637,8 +756,7 @@ extern "C" int vps_track_update(void* mem_feats, const void* det_feats, int dtyp
                                 const float* det_boxes, int32_t* mem_labels, const int32_t* det_labels,
                                 const int32_t* mem_src, int old_m, int cap, const int* new_m_dev, void* stream) {
   if (cap <= 0) return VPS_OK;
-  dim3 grid(8, cap);
-  VPS_DISPATCH_T(dtype, T, (track_update_kernel<T><<<grid, 256, 0, (cudaStream_t)stream>>>(
+  VPS_DISPATCH_T(dtype, T, (track_update_kernel<T><<<TU_BLOCKS, TU_THREADS, 0, (cudaStream_t)stream>>>(
                                (T*)mem_feats, (const T*)det_feats, feat_len, mem_boxes, det_boxes, mem_labels, det_labels,
                                mem_src, old_m, new_m_dev)));
   VPS_CUDA_LAST("track_update");

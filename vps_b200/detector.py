@@ -25,7 +25,6 @@ from .registry import (DETECTORS, build_backbone, build_extra_neck, build_head, 
                        build_roi_extractor)
 
 MAX_DET_CAP = 128      # detections kept per frame (config.test.max_det = 100, ties may exceed it)
-TRACK_CAP = 4096       # tracker memory slots
 
 
 def bbox2result_with_id(bboxes, labels, obj_ids):
@@ -87,14 +86,21 @@ class PanopticFuseTrack(nn.Module):
         if force:
             self._graphs.clear()          # captured graphs reference the old packed weights
             self._pf_queue, self._tail_done = [], [None, None]
+            self._emb_plan = None         # cached track embeddings were computed with the old weights
         for m in (self.backbone, self.neck, self.extra_neck, self.panopticFPN, self.rpn_head, self.bbox_head,
                   self.track_head, self.mask_head, self.flownet2):
             m.prepare(force)
         return self
 
     def reset_tracker(self):
+        """Tracker memory, as the reference keeps it (panoptic_fusetrack.py:391-469): every track opened since the first
+        frame of the clip, never evicted.  Slot j holds the RoI features, box and label of track j (prev_roi_feats,
+        prev_bboxes, prev_det_labels) and its track-head embedding (prev_emb, fp32 [cap, fc_out]), cached so that a frame
+        embeds only its own detections.  The buffers start at MAX_DET_CAP slots and double when a frame could outgrow
+        them; a slot costs 50 KB of fp32 (25 KB of bf16) RoI features plus 4 KB of embedding."""
         self.prev_n = 0
-        self.prev_roi_feats = self.prev_bboxes = self.prev_det_labels = None
+        self.prev_roi_feats = self.prev_bboxes = self.prev_det_labels = self.prev_emb = None
+        self._emb_plan = None             # (RoI feature dtype, tc32) under which prev_emb[:prev_n] was computed
 
     def extract_feat(self, x_nhwc):
         return self.neck(self.backbone(x_nhwc))
@@ -149,38 +155,63 @@ class PanopticFuseTrack(nn.Module):
         dev = det_boxes.device
         feat_len = det_roi_feats[0].numel()
         if self.prev_roi_feats is None or self.prev_roi_feats.dtype != det_roi_feats.dtype:
-            self.prev_roi_feats = torch.zeros((TRACK_CAP,) + tuple(det_roi_feats.shape[1:]), dtype=det_roi_feats.dtype, device=dev)
-            self.prev_bboxes = torch.zeros(TRACK_CAP, 4, device=dev)
-            self.prev_det_labels = torch.zeros(TRACK_CAP, dtype=torch.int32, device=dev)
-            self.prev_n = 0
+            self.reset_tracker()
+        if is_first:
+            self.prev_n = 0                                 # memory resets at the first frame of a clip (:400-406)
+        m = self.prev_n
+        self._reserve_tracks(m + k, det_roi_feats)          # a frame appends at most k tracks
+        cap = self.prev_bboxes.shape[0]
+        # the cached embeddings are those of the current weights and precision; embedding a row gives the same bits alone
+        # or in a batch of any size, so they equal a fresh embedding of the memory
+        plan = (det_roi_feats.dtype, ops.F32_TC[0])
+        if m > 0 and self._emb_plan != plan:
+            self.prev_emb[:m] = self.track_head.embed(self.prev_roi_feats[:m])
+        self._emb_plan = plan
+        emb = self.track_head.embed(det_roi_feats[:k])
+        assert emb.is_contiguous() or emb.stride(0) == emb.shape[1]
         ids = torch.empty(k, dtype=torch.int32, device=dev)
         new_m = torch.zeros(1, dtype=torch.int32, device=dev)
-        if is_first or self.prev_n == 0:
+        if m == 0:
             # ids = arange(k); memory := detections  (:400-406)
-            mem_src = torch.arange(TRACK_CAP, dtype=torch.int32, device=dev)      # host-built constant table
-            mem_src[k:] = -1
-            ids.copy_(mem_src[:k])
+            mem_src = torch.arange(k, dtype=torch.int32, device=dev)
+            ids.copy_(mem_src)
             new_m.fill_(k)
-            ops.track_update(self.prev_roi_feats, det_roi_feats, feat_len, self.prev_bboxes, det_boxes, self.prev_det_labels,
-                             det_labels, mem_src, 0, TRACK_CAP, new_m)
-            self.prev_n = k
-            return ids
-        m = self.prev_n
-        emb = self.track_head.embed(det_roi_feats[:k])
-        ref_emb = self.track_head.embed(self.prev_roi_feats[:m])
-        match_ids = torch.empty(k, dtype=torch.int32, device=dev)
-        comp = torch.empty(k, m + 1, device=dev)
-        mem_src = torch.empty(TRACK_CAP, dtype=torch.int32, device=dev)
-        ws = torch.empty((k * m + k + 2 * TRACK_CAP) * 4, dtype=torch.uint8, device=dev)
-        assert emb.is_contiguous() or emb.stride(0) == emb.shape[1]
-        ops.track_assign(emb, ref_emb, k, m, emb.shape[1], det_boxes, self.prev_bboxes, det_labels, self.prev_det_labels,
-                         cls_prob, self.track_head.match_coeff, TRACK_CAP, ids, match_ids, comp, mem_src, new_m, ws)
+        else:
+            match_ids = torch.empty(k, dtype=torch.int32, device=dev)
+            comp = torch.empty(k, m + 1, device=dev)
+            mem_src = torch.empty(cap, dtype=torch.int32, device=dev)
+            ws = torch.empty((k * m + k + 2 * cap) * 4, dtype=torch.uint8, device=dev)
+            ops.track_assign(emb, self.prev_emb[:m], k, m, emb.shape[1], det_boxes, self.prev_bboxes, det_labels,
+                             self.prev_det_labels, cls_prob, self.track_head.match_coeff, cap, ids, match_ids, comp, mem_src,
+                             new_m, ws)
+            if taps is not None:
+                taps.update(comp_scores=comp, match_ids=match_ids)
         ops.track_update(self.prev_roi_feats, det_roi_feats, feat_len, self.prev_bboxes, det_boxes, self.prev_det_labels,
-                         det_labels, mem_src, m, TRACK_CAP, new_m)
-        self.prev_n = int(new_m.item())                     # 4-byte read-back: tracker memory size
-        if taps is not None:
-            taps.update(comp_scores=comp, match_ids=match_ids)
+                         det_labels, mem_src, m, cap, new_m)
+        ops.track_update(self.prev_emb, emb, emb.shape[1], None, None, None, None, mem_src, m, cap, new_m)
+        self.prev_n = k if m == 0 else int(new_m.item())    # 4-byte read-back: tracker memory size
         return ids
+
+    def _reserve_tracks(self, n, det_roi_feats):
+        """Make the tracker memory hold at least n slots: allocate it at MAX_DET_CAP slots, then double; the first prev_n
+        slots are copied over on the current stream."""
+        cap = 0 if self.prev_bboxes is None else self.prev_bboxes.shape[0]
+        if n <= cap:
+            return
+        new_cap = max(cap, MAX_DET_CAP)
+        while new_cap < n:
+            new_cap *= 2
+        dev, m = det_roi_feats.device, self.prev_n
+        feats = torch.empty((new_cap,) + tuple(det_roi_feats.shape[1:]), dtype=det_roi_feats.dtype, device=dev)
+        boxes = torch.empty(new_cap, 4, device=dev)
+        labels = torch.empty(new_cap, dtype=torch.int32, device=dev)
+        emb = torch.empty(new_cap, self.track_head.fc_out_channels, device=dev)
+        if m > 0:
+            feats[:m] = self.prev_roi_feats[:m]
+            boxes[:m] = self.prev_bboxes[:m]
+            labels[:m] = self.prev_det_labels[:m]
+            emb[:m] = self.prev_emb[:m]
+        self.prev_roi_feats, self.prev_bboxes, self.prev_det_labels, self.prev_emb = feats, boxes, labels, emb
 
     # ------------------------------------------------------------------ static part + CUDA graph
     def _static_eager(self, img, ref_img, img_shape, taps=None, ref_feats=None):
