@@ -379,6 +379,10 @@ int vps_unify_pan(const void* seg, const void* pan, int label_bytes, int H, int 
 /* 1 if the last vps_unify_pan call on `ws` met a panoptic instance id without a cls_ind entry (the reference raises
  * IndexError there, cityscapes_vps.py:197); synchronises `stream` */
 int vps_unify_pan_error(const void* ws, void* stream);
+/* the image-level get_unified_pan_result of the image panoptic model (tools/dataset/base_dataset.py:232-274): the same
+ * histograms, decisions and workspace as vps_unify_pan, but no track ids, and the third output channel is 0 */
+int vps_unify_pan_image(const void* seg, const void* pan, int label_bytes, int H, int W, const int32_t* cls_ind, int k,
+                        int id_last_stuff, int stuff_area_limit, uint8_t* out, void* ws, int64_t ws_bytes, void* stream);
 int64_t vps_unify_pan_error_offset(void);   /* byte offset of that flag (int32) inside ws, for asynchronous read-back */
 
 /* ---- SURVEY 8f rank 2: pixel-level step of the VPQ evaluator (tools/eval_vpq.py:138-145) --------------------------

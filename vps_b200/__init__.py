@@ -1,4 +1,5 @@
-"""vps_b200: Hopper-native FuseTrack frame-pair path (drop-in modules for mcahny/vps's registries).
+"""vps_b200: Hopper-native inference for the reference's three Cityscapes models -- PanopticFuseTrack, PanopticTrack and
+PanopticFuse (drop-in modules for mcahny/vps's registries).
 
     from vps_b200 import Config, build_detector
     cfg = Config.fromfile('<reference>/configs/cityscapes/fusetrack.py')      # loads unmodified
@@ -11,5 +12,5 @@ from .registry import (BACKBONES, DETECTORS, EXTRA_NECKS, HEADS, LOSSES, NECKS, 
                        SHARED_HEADS, Registry, build_detector, build_from_cfg)
 from . import modules as _modules  # noqa: F401  (registers the classes)
 from . import detector as _detector  # noqa: F401
-from .detector import PanopticFuseTrack  # noqa: F401
-from .default_cfg import fusetrack_cfg  # noqa: F401
+from .detector import PanopticFuse, PanopticFuseTrack, PanopticTrack  # noqa: F401
+from .default_cfg import fuse_cfg, fusetrack_cfg, track_cfg  # noqa: F401

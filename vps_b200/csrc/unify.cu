@@ -1,4 +1,5 @@
-// SURVEY 8f rank 1: get_unified_pan_result (reference tools/dataset/cityscapes_vps.py:183-224) for one frame.
+// SURVEY 8f rank 1: get_unified_pan_result (reference tools/dataset/cityscapes_vps.py:183-224) for one frame, and its
+// image-level sibling (tools/dataset/base_dataset.py:232-274, vps_unify_pan_image).
 //
 // Everything the reference decides per REGION (= per panoptic id) depends only on two histograms: how many pixels each
 // panoptic id has, and, per id, how the semantic map votes inside it.  So the frame is processed as
@@ -87,8 +88,11 @@ __global__ void __launch_bounds__(256) unify_hist_kernel(const TL* __restrict__ 
 }
 
 // one block of NID threads; thread t decides the fate of panoptic id t
+// obj_mode: what the third channel holds -- OBJ_COPY (a copy of pan, the video function without track ids), OBJ_TRACK
+// (track id + 1) or OBJ_ZERO (the image-level function, tools/dataset/base_dataset.py:232-274, leaves it 0)
+enum { OBJ_COPY = 0, OBJ_TRACK = 1, OBJ_ZERO = 2 };
 __global__ void __launch_bounds__(NID) unify_decide_kernel(UnifyWs* __restrict__ ws, const __grid_constant__ UnifyIds ids,
-                                                           int has_obj, int k, int id_last_stuff,
+                                                           int obj_mode, int k, int id_last_stuff,
                                                            unsigned int stuff_area_limit) {
   __shared__ unsigned int s_area[NID];
   __shared__ int s_seg[NID];
@@ -121,7 +125,7 @@ __global__ void __launch_bounds__(NID) unify_decide_kernel(UnifyWs* __restrict__
         seg = winner; ins = 0; obj = 0;
       } else {
         seg = want & 255; ins = (rank + 1) & 255;
-        if (has_obj) obj = (ids.obj[rank < MAX_UNIFY_K ? rank : 0] + 1) & 255;   // looked up with the RANK, as the reference does (:201, :211)
+        if (obj_mode == OBJ_TRACK) obj = (ids.obj[rank < MAX_UNIFY_K ? rank : 0] + 1) & 255;   // looked up with the RANK, as the reference does (:201, :211)
       }
     }
   }
@@ -136,6 +140,7 @@ __global__ void __launch_bounds__(NID) unify_decide_kernel(UnifyWs* __restrict__
   }
   __syncthreads();
   if (seg <= id_last_stuff && s_kill[seg]) seg = 255;
+  if (obj_mode == OBJ_ZERO) obj = 0;
   ws->lut[t][0] = (unsigned char)seg; ws->lut[t][1] = (unsigned char)ins; ws->lut[t][2] = (unsigned char)obj; ws->lut[t][3] = 0;
 }
 
@@ -169,9 +174,9 @@ __global__ void __launch_bounds__(256) unify_apply_kernel(const TL* __restrict__
 
 extern "C" int64_t vps_unify_pan_ws_bytes(void) { return (int64_t)sizeof(UnifyWs); }
 
-extern "C" int vps_unify_pan(const void* seg, const void* pan, int label_bytes, int H, int W, const int32_t* cls_ind,
-                             const int32_t* obj_id, int k, int id_last_stuff, int stuff_area_limit, uint8_t* out, void* ws,
-                             int64_t ws_bytes, void* stream) {
+static int unify_pan(const void* seg, const void* pan, int label_bytes, int H, int W, const int32_t* cls_ind,
+                     const int32_t* obj_id, int obj_mode, int k, int id_last_stuff, int stuff_area_limit, uint8_t* out,
+                     void* ws, int64_t ws_bytes, void* stream) {
   VPS_CHECK_ARG(label_bytes == 1 || label_bytes == 8, "unify_pan: label_bytes %d", label_bytes);
   VPS_CHECK_ARG(ws_bytes >= (int64_t)sizeof(UnifyWs) && ((uintptr_t)ws & 15) == 0, "unify_pan: workspace");
   VPS_CHECK_ARG(id_last_stuff >= 0 && id_last_stuff < 255 && k >= 0 && k <= MAX_UNIFY_K && ((uintptr_t)out & 3) == 0, "unify_pan: args (k %d)", k);
@@ -189,12 +194,28 @@ extern "C" int vps_unify_pan(const void* seg, const void* pan, int label_bytes, 
   if (label_bytes == 1) unify_hist_kernel<uint8_t><<<blocks, 256, 0, st>>>((const uint8_t*)seg, (const uint8_t*)pan, npix, id_last_stuff, w);
   else unify_hist_kernel<int64_t><<<blocks, 256, 0, st>>>((const int64_t*)seg, (const int64_t*)pan, npix, id_last_stuff, w);
   VPS_CUDA_LAST("unify_hist");
-  unify_decide_kernel<<<1, NID, 0, st>>>(w, ids, obj_id != nullptr, k, id_last_stuff, (unsigned int)stuff_area_limit);
+  unify_decide_kernel<<<1, NID, 0, st>>>(w, ids, obj_mode, k, id_last_stuff, (unsigned int)stuff_area_limit);
   VPS_CUDA_LAST("unify_decide");
   if (label_bytes == 1) unify_apply_kernel<uint8_t><<<blocks, 256, 0, st>>>((const uint8_t*)pan, npix, w, out);
   else unify_apply_kernel<int64_t><<<blocks, 256, 0, st>>>((const int64_t*)pan, npix, w, out);
   VPS_CUDA_LAST("unify_apply");
   return VPS_OK;
+}
+
+extern "C" int vps_unify_pan(const void* seg, const void* pan, int label_bytes, int H, int W, const int32_t* cls_ind,
+                             const int32_t* obj_id, int k, int id_last_stuff, int stuff_area_limit, uint8_t* out, void* ws,
+                             int64_t ws_bytes, void* stream) {
+  return unify_pan(seg, pan, label_bytes, H, W, cls_ind, obj_id, obj_id ? OBJ_TRACK : OBJ_COPY, k, id_last_stuff,
+                   stuff_area_limit, out, ws, ws_bytes, stream);
+}
+
+// the image-level function (tools/dataset/base_dataset.py:232-274): same histograms and decisions, no track ids, and the
+// third channel stays 0
+extern "C" int vps_unify_pan_image(const void* seg, const void* pan, int label_bytes, int H, int W, const int32_t* cls_ind,
+                                   int k, int id_last_stuff, int stuff_area_limit, uint8_t* out, void* ws, int64_t ws_bytes,
+                                   void* stream) {
+  return unify_pan(seg, pan, label_bytes, H, W, cls_ind, nullptr, OBJ_ZERO, k, id_last_stuff, stuff_area_limit, out, ws,
+                   ws_bytes, stream);
 }
 
 // the reference raises IndexError when a panoptic instance id has no cls_ind entry (cityscapes_vps.py:197: cls_ind[id - id_last_stuff - 1]);

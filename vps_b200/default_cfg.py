@@ -1,6 +1,7 @@
-"""Built-in equivalent of the model / test_cfg sections of the reference's configs/cityscapes/fusetrack.py
-(lines 2-148) for environments where the reference tree is not mounted (the GPU box).  On a machine that has
-the reference, load its file instead: `Config.fromfile('<ref>/configs/cityscapes/fusetrack.py')`."""
+"""Built-in equivalents of the model / test_cfg sections of the reference's three Cityscapes configs
+(configs/cityscapes/fusetrack.py lines 2-148, track.py lines 2-135, fuse.py lines 2-142) for environments where the
+reference tree is not mounted.  On a machine that has the reference, load its file instead:
+`Config.fromfile('<ref>/configs/cityscapes/fusetrack.py')`."""
 
 
 def fusetrack_cfg():
@@ -34,3 +35,22 @@ def fusetrack_cfg():
         rcnn=dict(score_thr=0.05, nms=dict(type='nms', iou_thr=0.5), max_per_img=100, mask_thr_binary=0.5),
         loss_pano_weight=None, flownet2=[], class_mapping=cm)
     return dict(model=model, train_cfg=None, test_cfg=test_cfg)
+
+
+def track_cfg():
+    """configs/cityscapes/track.py: FuseTrack's model without the BFPTcea fuse neck, and no `flownet2` in test_cfg (so no
+    FlowNet2 either).  Its match_coeff spells the last weight as the integer 10."""
+    c = fusetrack_cfg()
+    c['model']['type'] = 'PanopticTrack'
+    del c['model']['extra_neck']
+    c['model']['track_head']['match_coeff'] = [1.0, 2.0, 10]
+    del c['test_cfg']['flownet2']
+    return c
+
+
+def fuse_cfg():
+    """configs/cityscapes/fuse.py: FuseTrack's model without the track head; the same test_cfg."""
+    c = fusetrack_cfg()
+    c['model']['type'] = 'PanopticFuse'
+    del c['model']['track_head']
+    return c

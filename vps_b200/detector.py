@@ -1,5 +1,13 @@
-"""PanopticFuseTrack on H100 -- the detector class the reference registers in DETECTORS
-(mmdet/models/detectors/panoptic_fusetrack.py:24-606), inference path.
+"""The reference's three Cityscapes detectors on H100, inference path, as it registers them in DETECTORS:
+  * PanopticFuseTrack (mmdet/models/detectors/panoptic_fusetrack.py:24-606, configs/cityscapes/fusetrack.py): FlowNet2 +
+    BFPTcea fuse neck over the (current, reference) pair, and the tracker;
+  * PanopticTrack (panoptic_track.py:21-536, configs/cityscapes/track.py): no flow, no fuse neck -- the current frame
+    only -- with the tracker;
+  * PanopticFuse (panoptic_fuse.py:23-473, configs/cityscapes/fuse.py): flow and fuse neck, no tracker -- the image
+    panoptic model.
+They share everything else (construction, weight preparation, the static part as one CUDA graph, the mask head /
+MaskRemoval / fusion tail, prefetch and forward_test) through `_PanopticDetector`; the subclasses only switch the flow +
+fuse neck (`with_flow`) and the tracker (`with_track`) on or off and shape the results.
 
 Construction follows TwoStageDetector.__init__ (two_stage.py:15-69): sub-modules are built from the
 config dicts through the registries, in the reference's order and under the reference's attribute
@@ -27,6 +35,13 @@ from .registry import (DETECTORS, build_backbone, build_extra_neck, build_head, 
 MAX_DET_CAP = 128      # detections kept per frame (config.test.max_det = 100, ties may exceed it)
 
 
+def bbox2result(bboxes, labels, num_classes):
+    """mmdet/core/bbox/transforms.py:138-156: one array of boxes per class."""
+    if bboxes.shape[0] == 0:
+        return [np.zeros((0, 5), dtype=np.float32) for _ in range(num_classes - 1)]
+    return [bboxes[labels == i, :] for i in range(num_classes - 1)]
+
+
 def bbox2result_with_id(bboxes, labels, obj_ids):
     """mmdet/core/bbox/transforms.py:159-180."""
     results = {}
@@ -38,8 +53,11 @@ def bbox2result_with_id(bboxes, labels, obj_ids):
     return results
 
 
-@DETECTORS.register_module
-class PanopticFuseTrack(nn.Module):
+class _PanopticDetector(nn.Module):
+    """What the three detectors share.  Subclasses set `with_flow` (FlowNet2 + fuse neck over the (current, reference)
+    pair) and `with_track` (the tracker) and build their results in `_results`."""
+    with_flow = True
+    with_track = True
     mean = [123.675, 116.28, 103.53]      # panoptic_fusetrack.py:92-93
     std = [58.395, 57.12, 57.375]
     # UPSNet globals read by MaskROI (tools/config/config.py:47,169) and ctor constants (:83-87)
@@ -50,14 +68,18 @@ class PanopticFuseTrack(nn.Module):
                  pretrained=None, precision="tc32"):
         super().__init__()
         assert shared_head is None
+        # the reference's configs hold exactly the modules each detector runs (track.py has no extra_neck, fuse.py no
+        # track_head), so the state_dict keys equal the reference model's
+        assert (extra_neck is not None) == self.with_flow, "extra_neck (BFPTcea) is given iff the detector fuses two frames"
+        assert (track_head is not None) == self.with_track, "track_head is given iff the detector tracks"
         self.backbone = build_backbone(backbone)
         self.neck = build_neck(neck)
-        self.extra_neck = build_extra_neck(extra_neck)
+        self.extra_neck = build_extra_neck(extra_neck) if self.with_flow else None
         self.panopticFPN = build_panoptic(panoptic)
         self.rpn_head = build_head(rpn_head)
         self.bbox_roi_extractor = build_roi_extractor(bbox_roi_extractor)
         self.bbox_head = build_head(bbox_head)
-        self.track_head = build_head(track_head)
+        self.track_head = build_head(track_head) if self.with_track else None
         self.mask_roi_extractor = build_roi_extractor(mask_roi_extractor)
         self.mask_head = build_head(mask_head)
         self.train_cfg, self.test_cfg = train_cfg, test_cfg
@@ -66,9 +88,16 @@ class PanopticFuseTrack(nn.Module):
         num_stuff = self.panopticFPN.num_stuff_classes
         assert self.class_mapping == {i: num_stuff - 1 + i for i in range(1, self.panopticFPN.num_things_classes + 1)}, \
             "the fused kernel assumes the Cityscapes thing->semantic mapping of fusetrack.py:148"
-        has_flow = (train_cfg is not None and 'flownet2' in train_cfg) or (test_cfg is not None and 'flownet2' in test_cfg)
-        assert has_flow, "Feature flow must be implemented."          # panoptic_fusetrack.py:513
-        self.flownet2 = FlowNet2(rgb_max=255.0)
+        # PanopticTrack and PanopticFuse take their panoptic branch on test_cfg.loss_pano_weight (panoptic_track.py:489,
+        # panoptic_fuse.py:443; without it Fuse would return semantic results only); its value is None, the reference
+        # tests the key
+        assert (self.with_flow and self.with_track) or (test_cfg is not None and 'loss_pano_weight' in test_cfg), \
+            "test_cfg must hold loss_pano_weight"
+        self.flownet2 = None
+        if self.with_flow:
+            has_flow = (train_cfg is not None and 'flownet2' in train_cfg) or (test_cfg is not None and 'flownet2' in test_cfg)
+            assert has_flow, "Feature flow must be implemented."          # panoptic_fusetrack.py:513
+            self.flownet2 = FlowNet2(rgb_max=255.0)
         self.precision = precision
         self.use_cuda_graph = True
         self.label_dtype = torch.int64        # dtype of the label maps: int64 as torch.max returns in the reference, or torch.uint8
@@ -89,7 +118,8 @@ class PanopticFuseTrack(nn.Module):
             self._emb_plan = None         # cached track embeddings were computed with the old weights
         for m in (self.backbone, self.neck, self.extra_neck, self.panopticFPN, self.rpn_head, self.bbox_head,
                   self.track_head, self.mask_head, self.flownet2):
-            m.prepare(force)
+            if m is not None:
+                m.prepare(force)
         return self
 
     def reset_tracker(self):
@@ -214,10 +244,20 @@ class PanopticFuseTrack(nn.Module):
         self.prev_roi_feats, self.prev_bboxes, self.prev_det_labels, self.prev_emb = feats, boxes, labels, emb
 
     # ------------------------------------------------------------------ static part + CUDA graph
-    def _static_eager(self, img, ref_img, img_shape, taps=None, ref_feats=None):
-        """ref_feats: FPN features (tuple of 5 NHWC maps) of the reference frame from an earlier call -- in a clip the
+    def _features(self, img, ref_img, taps=None, ref_feats=None):
+        """The pyramid the heads run on: (flow, x, ref_x, xf).  With the flow (FuseTrack, Fuse): FlowNet2 on the pair in
+        parallel with ResNet-50-FPN on both frames, then the BFPTcea fuse neck.
+        ref_feats: FPN features (tuple of 5 NHWC maps) of the reference frame from an earlier call -- in a clip the
         reference frame of frame t IS frame t - 1 (tools/dataset/cityscapes_vps.py:137-142), so its features were already
         computed as `x` of the previous pair; only the current frame then goes through ResNet-50-FPN."""
+        if not self.with_flow:
+            # current frame only (panoptic_track.py:447): one ResNet-50-FPN pass, its pyramid feeds the heads directly
+            _, _, H, W = img.shape
+            ops.SCOPE[0] = 'r50fpn'
+            x_in = empty_nhwc(1, H, W, 3, self.act_dtype, img.device)
+            ops.nchw_to_nhwc(img, x_in)
+            x = tuple(self.extract_feat(x_in))
+            return None, x, None, x
         dev = img.device
         _, _, H, W = img.shape
         dt = self.act_dtype
@@ -247,6 +287,11 @@ class PanopticFuseTrack(nn.Module):
         ref_x = tuple(f[1:2] for f in feats) if ref_feats is None else tuple(ref_feats)
         ops.SCOPE[0] = 'bfp_tcea'
         xf = self.extra_neck(x, ref_x, flow, taps)
+        return flow, x, ref_x, xf
+
+    def _static_eager(self, img, ref_img, img_shape, taps=None, ref_feats=None):
+        _, _, H, W = img.shape
+        flow, x, ref_x, xf = self._features(img, ref_img, taps, ref_feats)
         ops.SCOPE[0] = 'upsnet_fpn'
         nl = self.panopticFPN.num_levels
         # the semantic head and the RPN -> bbox head -> MaskROI chain both start from xf and meet only in the fusion tail
@@ -280,8 +325,12 @@ class PanopticFuseTrack(nn.Module):
             self._graphs[key] = "warm"
             return self._static_eager(img, ref_img, img_shape, None, ref_feats)
         if ent == "warm":
-            g_img, g_ref = torch.empty_like(img), torch.empty_like(ref_img)
-            g_img.copy_(img); g_ref.copy_(ref_img)
+            g_img = torch.empty_like(img)
+            g_img.copy_(img)
+            g_ref = None
+            if ref_img is not None:
+                g_ref = torch.empty_like(ref_img)
+                g_ref.copy_(ref_img)
             g_feats = None
             if cached:          # the graph reads the cached features from its own static buffers
                 g_feats = tuple(torch.empty_like(f) for f in ref_feats)
@@ -296,7 +345,8 @@ class PanopticFuseTrack(nn.Module):
             ops.lib().vps_add_launch_count(-ent[4])        # capture itself launched nothing
         graph, g_img, g_ref, outs, nlaunch, g_feats = ent
         g_img.copy_(img, non_blocking=True)
-        g_ref.copy_(ref_img, non_blocking=True)
+        if g_ref is not None:
+            g_ref.copy_(ref_img, non_blocking=True)
         if cached:
             for d_, s_ in zip(g_feats, ref_feats):
                 d_.copy_(s_, non_blocking=True)
@@ -307,7 +357,8 @@ class PanopticFuseTrack(nn.Module):
     @torch.no_grad()
     def prefetch(self, img, img_meta, ref_img=None, ref_feats=None):
         """Enqueue the static part (flow, backbones, necks, semantic head, RPN, bbox head, MaskROI -- everything that does
-        not depend on the tracker) of a FUTURE `simple_test(img, ...)` call on a side stream.  Two graph instances
+        not depend on the tracker) of a FUTURE `simple_test(img, ...)` call on a side stream.  A detector without the
+        flow (PanopticTrack) ignores ref_img and ref_feats.  Two graph instances
         ping-pong, so frame i+1's static part overlaps frame i's data-dependent tail and its host round-trips.  The
         matching simple_test call (same `img` object, in call order) picks the result up; results are identical."""
         if isinstance(ref_img, (list, tuple)):
@@ -326,28 +377,35 @@ class PanopticFuseTrack(nn.Module):
         st.wait_stream(cur)                                     # inputs are ready on the caller's stream
         if self._tail_done[slot] is not None:
             st.wait_event(self._tail_done[slot])                # the tail that last read this slot's outputs is done
+        if not self.with_flow:
+            ref_img = ref_feats = None                          # the current frame only
         with torch.cuda.stream(st):
             a = img.contiguous().float()
-            b = ref_img.contiguous().float()
+            b = ref_img.contiguous().float() if ref_img is not None else None
             outs = self._static_part(a, b, tuple(meta['img_shape'][:2]), True, None, slot, ref_feats)
             ev = torch.cuda.Event()
             ev.record(st)
         img.record_stream(st)
-        ref_img.record_stream(st)
+        if ref_img is not None:
+            ref_img.record_stream(st)
         self._pf_queue.append((img, slot, outs, ev))
 
     # ------------------------------------------------------------------ the hot path
     @torch.no_grad()
     def simple_test(self, img, img_meta, proposals=None, rescale=False, ref_img=None, taps=None, ref_feats=None):
-        """panoptic_fusetrack.py:502-606.  img / ref_img: NCHW fp32 CUDA tensors [1,3,H,W] (ref_img may be the
-        one-element list the reference's collate produces).  Returns (bbox_results, segm_results, pano_results).
+        """panoptic_fusetrack.py:502-606, panoptic_track.py:443-536, panoptic_fuse.py:399-473.  img / ref_img: NCHW fp32
+        CUDA tensors [1,3,H,W] (ref_img may be the one-element list the reference's collate produces; PanopticTrack
+        accepts and ignores it).  Returns (bbox_results, segm_results, pano_results).
         ref_feats: optional cached FPN features of ref_img (pano_results['fpn_feats'] of the call that had ref_img as its
         current frame): skips the reference frame's ResNet-50-FPN pass, results are bit-identical."""
         assert proposals is None
         if isinstance(ref_img, (list, tuple)):
             ref_img = ref_img[0]
+        if not self.with_flow:
+            ref_img = ref_feats = None                                 # panoptic_track.py:443-447: the current frame only
         meta = img_meta[0] if isinstance(img_meta, (list, tuple)) else img_meta
-        assert 'city' in meta['filename'] and 'iid' in meta            # :375
+        if self.with_track:
+            assert 'city' in meta['filename'] and 'iid' in meta        # :375
         self.prepare()
         assert self.precision in ("tc32", "bf16", "fp32"), self.precision
         ops.F32_TC[0] = self.precision == "tc32"
@@ -356,7 +414,8 @@ class PanopticFuseTrack(nn.Module):
         assert n == 1
         img_arg = img
         img = img.contiguous().float()
-        ref_img = ref_img.contiguous().float()
+        if ref_img is not None:
+            ref_img = ref_img.contiguous().float()
         # ---- static part (flow, backbones, fuse neck, semantic head, RPN, bbox head, MaskROI): fixed shapes, no host
         # decisions -> replayed as ONE CUDA graph after the first eager call for this (shape, precision)
         use_graph = self.use_cuda_graph and taps is None and ops.PROFILE is None
@@ -381,14 +440,16 @@ class PanopticFuseTrack(nn.Module):
         if self.precision == "tc32" and ops.tc32_overflow():
             raise ops.VpsError("tc32: an activation or weight exceeded the fp16 range (65504) of the main tensor-core "
                                "product; use precision='fp32' for this input")
-        iid = meta['iid']
-        is_first = (iid % 10000) == 1
-        det_roi_feats = self.bbox_roi_extractor(xf, det_rois, k)
+        det_roi_feats = det_obj_ids = None
+        if self.with_track:
+            det_roi_feats = self.bbox_roi_extractor(xf, det_rois, k)
         det_boxes_c = torch.empty(MAX_DET_CAP, 4, device=dev)
         det_labels = torch.empty(MAX_DET_CAP, dtype=torch.int32, device=dev)
         ops.det_split(det_rois, cls_idx, MAX_DET_CAP, det_boxes_c, det_labels)
         cls_idx_h = cls_idx[:k].cpu().numpy()
-        det_obj_ids = self._track(det_roi_feats, det_boxes_c, det_labels, cls_prob, k, is_first, taps)
+        if self.with_track:
+            is_first = (meta['iid'] % 10000) == 1
+            det_obj_ids = self._track(det_roi_feats, det_boxes_c, det_labels, cls_prob, k, is_first, taps)
 
         # ---- mask head on the detections (:561-568)
         mask_feats = self.mask_roi_extractor(xf, det_rois, k)
@@ -421,23 +482,12 @@ class PanopticFuseTrack(nn.Module):
             keep_h = np.array([0], dtype=np.int64)           # mask_removal.py:52-54,89-91
         det_rois_h = det_rois[:k].cpu().numpy()
         cls_prob_h = cls_prob[:k].cpu().numpy()
-        ids_h = det_obj_ids[:k].cpu().numpy()
-        labels_h = cls_idx_h - 1
+        ids_h = det_obj_ids[:k].cpu().numpy() if self.with_track else None
         h0, w0 = meta['img_shape'][:2]
-        pano_results = {
-            'fcn_outputs': sem[None, :h0, :w0],
-            'panoptic_cls_inds': torch.from_numpy(cls_idx_h[keep_h].astype(np.int64)).to(dev),
-            'panoptic_cls_prob': torch.from_numpy(cls_prob_h[keep_h]).to(dev),
-            'panoptic_det_labels': torch.from_numpy(labels_h[keep_h].astype(np.int64)).to(dev),
-            'panoptic_det_obj_ids': torch.from_numpy(ids_h[keep_h]).to(dev),
-            'panoptic_outputs': pano[None, :h0, :w0],
-            # host copies of the two small per-instance arrays (already on the host here): the post-processing that follows
-            # the path (vps_b200.postproc.PanUnifier) needs them there
-            'host': dict(panoptic_cls_inds=cls_idx_h[keep_h].astype(np.int64), panoptic_det_obj_ids=ids_h[keep_h]),
-            # FPN features of the current frame: a streaming caller hands them back as `ref_feats` of the next pair
-            'fpn_feats': x,
-        }
-        bbox_results = bbox2result_with_id(det_rois_h[:, 1:], labels_h, ids_h)
+        bbox_results, pano_results = self._results(det_rois_h, cls_idx_h, cls_prob_h, ids_h, keep_h,
+                                                   sem[None, :h0, :w0], pano[None, :h0, :w0], dev)
+        # FPN features of the current frame: a streaming caller hands them back as `ref_feats` of the next pair
+        pano_results['fpn_feats'] = x
         segm_results = [[] for _ in range(self.mask_head.num_classes - 1)]     # :484-485 (`or True`)
         if taps is not None:
             taps.update(flow=flow, fpn=x, ref_fpn=ref_x, fused=xf, fcn_score=fcn_score, fcn_output=fcn_output,
@@ -450,6 +500,23 @@ class PanopticFuseTrack(nn.Module):
             done.record(torch.cuda.current_stream(dev))
             self._tail_done[pf_slot] = done
         return bbox_results, segm_results, pano_results
+
+    def _results(self, det_rois_h, cls_idx_h, cls_prob_h, ids_h, keep_h, sem, pano, dev):
+        """(bbox_results, pano_results) of the tracking detectors (panoptic_fusetrack.py:598-606, panoptic_track.py:
+        474-475, 527-534): boxes keyed by track id, and the kept instances with their labels and track ids."""
+        labels_h = cls_idx_h - 1
+        pano_results = {
+            'fcn_outputs': sem,
+            'panoptic_cls_inds': torch.from_numpy(cls_idx_h[keep_h].astype(np.int64)).to(dev),
+            'panoptic_cls_prob': torch.from_numpy(cls_prob_h[keep_h]).to(dev),
+            'panoptic_det_labels': torch.from_numpy(labels_h[keep_h].astype(np.int64)).to(dev),
+            'panoptic_det_obj_ids': torch.from_numpy(ids_h[keep_h]).to(dev),
+            'panoptic_outputs': pano,
+            # host copies of the two small per-instance arrays (already on the host here): the post-processing that follows
+            # the path (vps_b200.postproc.PanUnifier) needs them there
+            'host': dict(panoptic_cls_inds=cls_idx_h[keep_h].astype(np.int64), panoptic_det_obj_ids=ids_h[keep_h]),
+        }
+        return bbox2result_with_id(det_rois_h[:, 1:], labels_h, ids_h), pano_results
 
     # reference-compatible entry (base.py:79-104)
     def forward_test(self, imgs, img_metas, **kwargs):
@@ -465,3 +532,34 @@ class PanopticFuseTrack(nn.Module):
         if return_loss:
             raise NotImplementedError("forward_train: training path is a later scope row (SURVEY 8f rank 3)")
         return self.forward_test(img, img_meta, **kwargs)
+
+
+@DETECTORS.register_module
+class PanopticFuseTrack(_PanopticDetector):
+    """VPSNet-FuseTrack (panoptic_fusetrack.py, configs/cityscapes/fusetrack.py): flow, fuse neck and tracker."""
+
+
+@DETECTORS.register_module
+class PanopticTrack(_PanopticDetector):
+    """VPSNet-Track (panoptic_track.py, configs/cityscapes/track.py): the current frame only -- no FlowNet2, no fuse
+    neck, no reference-frame backbone pass -- with the tracker.  `ref_img` is accepted and ignored."""
+    with_flow = False
+
+
+@DETECTORS.register_module
+class PanopticFuse(_PanopticDetector):
+    """VPSNet-Fuse, the image panoptic model (panoptic_fuse.py, configs/cityscapes/fuse.py): flow and fuse neck, no
+    tracker.  bbox_results are per-class box arrays (bbox2result), pano_results carry no track ids or labels."""
+    with_track = False
+
+    def _results(self, det_rois_h, cls_idx_h, cls_prob_h, ids_h, keep_h, sem, pano, dev):
+        """panoptic_fuse.py:413-414, 463-469."""
+        cls_k = cls_idx_h[keep_h].astype(np.int64)
+        pano_results = {
+            'fcn_outputs': sem,
+            'panoptic_cls_inds': torch.from_numpy(cls_k).to(dev),
+            'panoptic_cls_prob': torch.from_numpy(cls_prob_h[keep_h]).to(dev),
+            'panoptic_outputs': pano,
+            'host': dict(panoptic_cls_inds=cls_k),
+        }
+        return bbox2result(det_rois_h[:, 1:], cls_idx_h - 1, self.bbox_head.num_classes), pano_results

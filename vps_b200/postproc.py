@@ -3,7 +3,10 @@
 
 `PanUnifier` mirrors the reference method: call it once per frame, in clip order, with the label maps and the
 `panoptic_cls_inds` / `panoptic_det_obj_ids` of `simple_test`; it returns the uint8 [H,W,3] (semantic, instance rank,
-track id + 1) image the VPQ writer consumes.  The only host-side state is the reference's duplicate-track-id counter."""
+track id + 1) image the VPQ writer consumes.  The only host-side state is the reference's duplicate-track-id counter.
+
+`PanUnifier(image=True)` is the image-level function the image panoptic model (PanopticFuse) is evaluated with
+(tools/dataset/base_dataset.py:232-274): the same regions and decisions, no track ids, no counter, third channel 0."""
 import ctypes as C
 
 import numpy as np
@@ -14,8 +17,9 @@ from ._lib import lib
 
 
 class PanUnifier:
-    def __init__(self, num_seg_classes=19, num_classes=9, stuff_area_limit=4 * 64 * 64):
+    def __init__(self, num_seg_classes=19, num_classes=9, stuff_area_limit=4 * 64 * 64, image=False):
         # configs/cityscapes/test_cityscapes_1gpu.yaml:7-8; cityscapes_vps.py:162 (stuff_area_limit), :166 (max_oid)
+        self.image = image
         self.id_last_stuff = num_seg_classes - num_classes
         self.stuff_area_limit = stuff_area_limit
         self.max_oid = 100
@@ -49,7 +53,7 @@ class PanUnifier:
     @torch.no_grad()
     def __call__(self, seg, pan, cls_ind, obj_id=None, out=None):
         """seg, pan: CUDA label maps [H,W] or [1,H,W] (uint8 or int64); cls_ind, obj_id: per-instance arrays (tensor /
-        numpy / list).  Returns a uint8 CUDA tensor [H,W,3]."""
+        numpy / list); obj_id must be None for the image-level function.  Returns a uint8 CUDA tensor [H,W,3]."""
         if not (seg.is_cuda and pan.is_cuda):
             raise RuntimeError("PanUnifier: label maps must be CUDA tensors (there is no CPU path)")
         seg = seg.reshape(seg.shape[-2:]).contiguous()
@@ -60,6 +64,8 @@ class PanUnifier:
         cls_np = np.ascontiguousarray(np.asarray(cls_ind.cpu() if torch.is_tensor(cls_ind) else cls_ind).reshape(-1), dtype=np.int32)
         k = int(cls_np.shape[0])
         obj_np = None
+        if self.image and obj_id is not None:
+            raise ValueError("PanUnifier(image=True): the image-level result has no track ids")
         if obj_id is not None:
             obj_np = np.asarray(obj_id.cpu() if torch.is_tensor(obj_id) else obj_id).reshape(-1)
             obj_np = np.ascontiguousarray(self.dedup_track_ids(obj_np), dtype=np.int32)
@@ -70,7 +76,12 @@ class PanUnifier:
             self._ws = torch.empty(int(lib().vps_unify_pan_ws_bytes()), dtype=torch.uint8, device=dev)
         if out is None:
             out = torch.empty(H, W, 3, dtype=torch.uint8, device=dev)
-        ops.check(lib().vps_unify_pan(ops._ptr(seg), ops._ptr(pan), seg.element_size(), H, W, cls_p, obj_p, k,
-                                      self.id_last_stuff, self.stuff_area_limit, ops._ptr(out), ops._ptr(self._ws),
-                                      C.c_int64(self._ws.numel()), ops.stream()), "unify_pan")
+        if self.image:
+            ops.check(lib().vps_unify_pan_image(ops._ptr(seg), ops._ptr(pan), seg.element_size(), H, W, cls_p, k,
+                                                self.id_last_stuff, self.stuff_area_limit, ops._ptr(out), ops._ptr(self._ws),
+                                                C.c_int64(self._ws.numel()), ops.stream()), "unify_pan_image")
+        else:
+            ops.check(lib().vps_unify_pan(ops._ptr(seg), ops._ptr(pan), seg.element_size(), H, W, cls_p, obj_p, k,
+                                          self.id_last_stuff, self.stuff_area_limit, ops._ptr(out), ops._ptr(self._ws),
+                                          C.c_int64(self._ws.numel()), ops.stream()), "unify_pan")
         return out

@@ -11,7 +11,11 @@ around the model call made asynchronous:
     graph instances ping-pong) is enqueued before the current pair's data-dependent tail, so the tail and its host
     round-trips overlap the next pair's graph.
 
-Nothing about the model call changes: `det.simple_test` is the same entry the parity tests use."""
+Nothing about the model call changes: `det.simple_test` is the same entry the parity tests use.
+
+The loop serves all three detectors.  PanopticTrack reads the current frame only: its pairs are `(img, None)`, and no
+reference frame is uploaded or normalised.  PanopticFuse has no tracker: with `unify` it gets the image-level unified
+result (`PanUnifier(image=True)`)."""
 import torch
 
 
@@ -29,11 +33,12 @@ class ClipRunner:
         self.streaming = streaming
         self._prev_feats = None
         # unify: also run get_unified_pan_result (tools/dataset/cityscapes_vps.py:162-226) on the GPU for every pair
-        # (vps_b200.postproc.PanUnifier) and return the uint8 [H,W,3] image as pano_results['pan_2ch'] (host)
+        # (vps_b200.postproc.PanUnifier) and return the uint8 [H,W,3] image as pano_results['pan_2ch'] (host); a detector
+        # without a tracker gets the image-level function (tools/dataset/base_dataset.py:232-274)
         self.unifier = None
         if unify:
             from .postproc import PanUnifier
-            self.unifier = PanUnifier()
+            self.unifier = PanUnifier(image=not det.with_track)
         self._out2 = []
         self._err = None
         self.dev = torch.device(device) if device is not None else next(det.parameters()).device
@@ -51,12 +56,14 @@ class ClipRunner:
         while len(self._in) <= slot:
             self._in.append(None)
         bufs = self._in[slot]
-        if bufs is None or bufs[0].shape != pair[0].shape or bufs[0].dtype != pair[0].dtype:
-            bufs = self._in[slot] = (torch.empty(pair[0].shape, dtype=pair[0].dtype, device=self.dev),
-                                     torch.empty(pair[1].shape, dtype=pair[1].dtype, device=self.dev))
+        if bufs is None or any((b is None) != (p is None) or (p is not None and (b.shape != p.shape or b.dtype != p.dtype))
+                               for b, p in zip(bufs, pair)):
+            bufs = self._in[slot] = tuple(None if p is None else torch.empty(p.shape, dtype=p.dtype, device=self.dev)
+                                          for p in pair[:2])
         with torch.cuda.stream(self.copy):
-            bufs[0].copy_(pair[0], non_blocking=True)
-            bufs[1].copy_(pair[1], non_blocking=True)
+            for b, p in zip(bufs, pair):
+                if p is not None:                           # (img, None): a detector that reads the current frame only
+                    b.copy_(p, non_blocking=True)
             ev = torch.cuda.Event()
             ev.record(self.copy)
         return bufs[0], bufs[1], ev
@@ -76,11 +83,12 @@ class ClipRunner:
         """enqueue the static part of a pair; in streaming mode the previous ENQUEUED pair's features are its reference
         features (they are produced on the same side stream, in order)"""
         feats = None
+        ref = [staged[1]] if staged[1] is not None else None
         if self.streaming and (meta['iid'] % 10000) != 1 and self.det._pf_queue:
             feats = self.det._pf_queue[-1][2]['x']
         elif self.streaming and (meta['iid'] % 10000) != 1:
             feats = self._prev_feats
-        self.det.prefetch(staged[0], [meta], ref_img=[staged[1]], ref_feats=feats)
+        self.det.prefetch(staged[0], [meta], ref_img=ref, ref_feats=feats)
         if self.streaming:
             self._prev_feats = self.det._pf_queue[-1][2]['x'] if self.det._pf_queue else None
 
@@ -92,6 +100,9 @@ class ClipRunner:
             self._f32.append([None, None])
         outs = []
         for k in (0, 1):
+            if staged[k] is None:
+                outs.append(None)
+                continue
             o, _ = self.input_stage(staged[k], out=self._f32[slot][k] if (self._f32[slot][k] is not None and
                                                                             self._f32[slot][k].shape[2] >= staged[k].shape[0]) else None)
             self._f32[slot][k] = o
@@ -105,7 +116,8 @@ class ClipRunner:
         return self._upload(pair)
 
     def run(self, pairs, metas, resident=False, prefetch=True):
-        """pairs: iterable of (img, ref_img) pinned host tensors [1,3,H,W] fp32 (device tensors if `resident`); metas:
+        """pairs: iterable of (img, ref_img) pinned host tensors [1,3,H,W] fp32 (device tensors if `resident`; ref_img is
+        None for a detector that reads the current frame only, PanopticTrack); metas:
         matching img_meta dicts.  Yields (bbox_results, segm_results, pano_results) per pair, in order;
         pano_results['panoptic_outputs'] and ['fcn_outputs'] are HOST tensors in a ring of depth + 1 pinned buffers: the
         download of pair i + depth + 1 reuses the slot of pair i and is issued right before result i + depth is yielded, so a
@@ -140,11 +152,12 @@ class ClipRunner:
                     staged = self._normalise(staged)
                 if prefetch:
                     self._prefetch(staged, cur[1])
+            rb = [b] if b is not None else None
             if prefetch or not self.streaming:
-                r = self.det.simple_test(a, [meta], ref_img=[b])
+                r = self.det.simple_test(a, [meta], ref_img=rb)
             else:
                 first = (meta['iid'] % 10000) == 1
-                r = self.det.simple_test(a, [meta], ref_img=[b], ref_feats=None if first else self._prev_feats)
+                r = self.det.simple_test(a, [meta], ref_img=rb, ref_feats=None if first else self._prev_feats)
                 self._prev_feats = r[2]['fpn_feats']
             pano, sem = r[2]["panoptic_outputs"], r[2]["fcn_outputs"]
             p2 = None
