@@ -399,6 +399,19 @@ int vps_rgb_to_id(const uint8_t* rgb, int64_t npix, uint32_t* ids, void* stream)
  * (semantic < num_stuff: id 1000 * semantic + 1, whatever the track channel holds), one per (thing category, track) key
  * (id 1000 * semantic + track + 1), VOID (semantic 255) -> 0 */
 int vps_pan2ch_ids(const uint8_t* pan_2ch, int64_t npix, int num_stuff, uint32_t* ids, void* stream);
+/* the same for the image-level unified result (vps_unify_pan_image) and the image converter _converter_2ch_single_core
+ * (tools/dataset/base_dataset.py:287-335), which keys segments by 1000 * semantic + instance rank (channel 1): id
+ * 1000 * semantic + instance + 1 for things, 1000 * semantic + 1 for stuff (the image unify leaves channel 1 at 0 there),
+ * VOID -> 0 */
+int vps_pan2ch_image_ids(const uint8_t* pan_2ch, int64_t npix, int num_stuff, uint32_t* ids, void* stream);
+
+/* ---- semantic mIoU of the reference (Cityscapes.evaluate_ssegs, tools/dataset/cityscapes.py:112-166) ----------------
+ * ADDS the confusion counts of one frame into conf (device uint64 [num_classes * num_classes], row = gt): index
+ * gt * C + pred over the pixels with gt != 255, counted iff index < C * C (np.bincount + the reference's copy loop,
+ * base_dataset.py:449-467; a pred >= C aliases into the next row).  gt: device uint8 trainIds [npix]; pred: device label
+ * map of label_bytes 1 (uint8) or 8 (int64, low byte used).  num_classes <= 64. */
+int vps_seg_confusion(const uint8_t* gt, const void* pred, int label_bytes, int64_t npix, int num_classes, uint64_t* conf,
+                      void* stream);
 
 /* ---- input stage (SURVEY 8f rank 4) -----------------------------------------------------------------------------------------
  * Normalize (mmcv.imnormalize: float32, BGR->RGB, (x - mean) / std; transforms.py:295-318) + Pad(size_divisor) (zero pad bottom /

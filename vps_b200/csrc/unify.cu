@@ -10,7 +10,7 @@
 // Bit-exact with the reference's numpy (uint8 wrap-around included); no per-region passes, no host round trip.
 #include <stddef.h>
 
-#include "common.cuh"
+#include "label_runs.cuh"
 
 namespace {
 constexpr int NID = 256;            // panoptic ids are uint8 in the reference (test_vpq.py:52-56)
@@ -30,11 +30,9 @@ struct UnifyWs {
   int error;
 };
 
-template <typename TL>
-__device__ __forceinline__ int lab(const TL* p, int64_t i) { return (int)((unsigned long long)p[i] & 0xFFull); }
+using vps::lab;
 
-// label maps are piecewise constant: every thread walks a run of 16 consecutive pixels and issues one shared-memory
-// atomic per (pan, seg) run instead of one per pixel
+// one shared-memory atomic per run of equal (pan, seg) labels in a 16-pixel strip (label_runs.cuh)
 template <typename TL>
 __global__ void __launch_bounds__(256) unify_hist_kernel(const TL* __restrict__ seg, const TL* __restrict__ pan, int64_t npix,
                                                          int id_last_stuff, UnifyWs* __restrict__ ws) {
@@ -52,32 +50,7 @@ __global__ void __launch_bounds__(256) unify_hist_kernel(const TL* __restrict__ 
       else atomicAdd(&ws->vote[p][sg], n);
     }
   };
-  constexpr int RUN = 16;
-  const int64_t nrun = (npix + RUN - 1) / RUN;
-  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < nrun; r += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t i0 = r * RUN;
-    const int cnt = (int)min((int64_t)RUN, npix - i0);
-    int pv[RUN], sv[RUN];
-    if (sizeof(TL) == 1 && cnt == RUN && ((i0 & 15) == 0) && ((((uintptr_t)pan) | ((uintptr_t)seg)) & 15) == 0) {
-      const uint4 a = *reinterpret_cast<const uint4*>((const uint8_t*)pan + i0);
-      const uint4 b = *reinterpret_cast<const uint4*>((const uint8_t*)seg + i0);
-      const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-      for (int e = 0; e < RUN; ++e) { pv[e] = (aw[e >> 2] >> (8 * (e & 3))) & 255; sv[e] = (bw[e >> 2] >> (8 * (e & 3))) & 255; }
-    } else {
-#pragma unroll
-      for (int e = 0; e < RUN; ++e) { pv[e] = e < cnt ? lab(pan, i0 + e) : -1; sv[e] = e < cnt ? lab(seg, i0 + e) : -1; }
-    }
-    int cp = pv[0], cs = sv[0];
-    unsigned int n = 1;
-#pragma unroll
-    for (int e = 1; e < RUN; ++e) {
-      if (pv[e] < 0) break;
-      if (pv[e] == cp && sv[e] == cs) { ++n; }
-      else { flush(cp, cs, n); cp = pv[e]; cs = sv[e]; n = 1; }
-    }
-    flush(cp, cs, n);
-  }
+  vps::walk_label_runs(pan, seg, npix, flush);
   __syncthreads();
   for (int i = threadIdx.x; i < NID; i += blockDim.x)
     if (s_area[i]) atomicAdd(&ws->area[i], s_area[i]);

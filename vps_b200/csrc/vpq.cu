@@ -24,11 +24,24 @@ __global__ void rgb_to_id_kernel(const uint8_t* __restrict__ rgb, int64_t n, uin
 // a stuff category (the native stuff pixels carry their pan value in the track channel, a thing region demoted to stuff
 // carries 0) collapses into ONE segment per frame -- and one colour per (thing category, track) key, kept across frames.
 // Deterministic stand-in for the colours: stuff -> 1000 * semantic + 1, thing -> 1000 * semantic + track + 1, VOID -> 0.
+// KEY_CH = 2 is that video converter.  KEY_CH = 1 is the image converter (tools/dataset/base_dataset.py:287-335), which
+// keys pixels by 1000 * semantic + instance rank: one segment per thing instance, and, since the image-level unify leaves
+// the instance channel 0 on every stuff pixel, one per stuff category.
+template <int KEY_CH>
 __global__ void pan2ch_ids_kernel(const uint8_t* __restrict__ p2, int64_t n, uint32_t num_stuff, uint32_t* __restrict__ ids) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const uint32_t sem = p2[3 * i], trk = p2[3 * i + 2];
-    ids[i] = sem == 255u ? 0u : 1000u * sem + (sem < num_stuff ? 0u : trk) + 1u;
+    const uint32_t sem = p2[3 * i], key = p2[3 * i + KEY_CH];
+    ids[i] = sem == 255u ? 0u : 1000u * sem + (sem < num_stuff ? 0u : key) + 1u;
   }
+}
+
+template <int KEY_CH>
+int pan2ch_ids(const uint8_t* pan_2ch, int64_t npix, int num_stuff, uint32_t* ids, void* stream) {
+  if (npix <= 0) return VPS_OK;
+  const int blocks = (int)((npix + 255) / 256 > 148 * 16 ? 148 * 16 : (npix + 255) / 256);
+  pan2ch_ids_kernel<KEY_CH><<<blocks, 256, 0, (cudaStream_t)stream>>>(pan_2ch, npix, (uint32_t)num_stuff, ids);
+  VPS_CUDA_LAST("pan2ch_ids");
+  return VPS_OK;
 }
 
 struct Layout { size_t keys, sorted, temp, temp_bytes, total; };
@@ -52,11 +65,11 @@ Layout layout(int64_t n, int cap) {
 extern "C" int64_t vps_tube_confusion_ws_bytes(int64_t npix) { return npix > 0 ? (int64_t)layout(npix, 0).total : 256; }
 
 extern "C" int vps_pan2ch_ids(const uint8_t* pan_2ch, int64_t npix, int num_stuff, uint32_t* ids, void* stream) {
-  if (npix <= 0) return VPS_OK;
-  const int blocks = (int)((npix + 255) / 256 > 148 * 16 ? 148 * 16 : (npix + 255) / 256);
-  pan2ch_ids_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(pan_2ch, npix, (uint32_t)num_stuff, ids);
-  VPS_CUDA_LAST("pan2ch_ids");
-  return VPS_OK;
+  return pan2ch_ids<2>(pan_2ch, npix, num_stuff, ids, stream);
+}
+
+extern "C" int vps_pan2ch_image_ids(const uint8_t* pan_2ch, int64_t npix, int num_stuff, uint32_t* ids, void* stream) {
+  return pan2ch_ids<1>(pan_2ch, npix, num_stuff, ids, stream);
 }
 
 extern "C" int vps_rgb_to_id(const uint8_t* rgb, int64_t npix, uint32_t* ids, void* stream) {

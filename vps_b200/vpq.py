@@ -90,6 +90,69 @@ def _merge_segments(seg_list):
     return out
 
 
+def recount_pred_areas(pred_segms, pred_segments, pairs, counts, categories):
+    """Predicted areas recounted from the id map, with the reference's sanity checks (eval_vpq.py:102-116,
+    base_dataset.py:352-366): pred_segms (id -> segment, updated in place) from the list pred_segments; (pairs, counts) =
+    the frame's sorted (gt * 2^24 + pred) codes and their pixel counts."""
+    area = defaultdict(int)
+    for lab, c in zip((pairs % np.uint64(OFFSET)).tolist(), counts.tolist()):
+        area[lab] += c
+    left = set(el["id"] for el in pred_segments)
+    for lab in sorted(area):
+        if lab not in pred_segms:
+            if lab == VOID:
+                continue
+            raise KeyError("Segment with ID {} is presented in PNG and not presented in JSON.".format(lab))
+        pred_segms[lab]["area"] = area[lab]
+        left.remove(lab)
+        if pred_segms[lab]["category_id"] not in categories:
+            raise KeyError("Segment with ID {} has unknown category_id {}.".format(lab, pred_segms[lab]["category_id"]))
+    if left:
+        raise KeyError("The following segment IDs {} are presented in JSON and not presented in PNG.".format(sorted(left)))
+
+
+def match_segments(stat, gt_segms, pred_segms, gt_pred, check_iou):
+    """The matching of the reference's PQ cores (eval_vpq.py:157-207 for a tube, base_dataset.py:378-431 for an image):
+    gt_segms / pred_segms map id -> segment (area, category_id, iscrowd), gt_pred maps (gt id, pred id) -> intersection in
+    ascending key order.  A match needs a non-crowd gt of the same category and IoU > 0.5, with the prediction's VOID pixels
+    removed from the union; an unmatched gt is a false negative unless it is crowd; an unmatched prediction is a false
+    positive unless more than half of it lies on VOID or on the crowd region of its category.  check_iou: the VPQ core's
+    `iou <= 1` assertion (the image core has none).  Adds into stat (category -> CatStat) in the reference's order."""
+    gt_matched, pred_matched = set(), set()
+    for (g, p), inter in gt_pred.items():
+        if g not in gt_segms or p not in pred_segms:
+            continue
+        if gt_segms[g]["iscrowd"] == 1 or gt_segms[g]["category_id"] != pred_segms[p]["category_id"]:
+            continue
+        union = pred_segms[p]["area"] + gt_segms[g]["area"] - inter - gt_pred.get((VOID, p), 0)
+        iou = inter / union
+        if check_iou:
+            assert iou <= 1.0, "INVALID IOU VALUE : %d" % g
+        if iou > 0.5:
+            c = stat[gt_segms[g]["category_id"]]
+            c.tp += 1
+            c.iou += iou
+            gt_matched.add(g)
+            pred_matched.add(p)
+    crowd = {}
+    for g, info in gt_segms.items():
+        if g in gt_matched:
+            continue
+        if info["iscrowd"] == 1:
+            crowd[info["category_id"]] = g
+            continue
+        stat[info["category_id"]].fn += 1
+    for p, info in pred_segms.items():
+        if p in pred_matched:
+            continue
+        inter = gt_pred.get((VOID, p), 0)
+        if info["category_id"] in crowd:
+            inter += gt_pred.get((crowd[info["category_id"]], p), 0)
+        if inter / info["area"] > 0.5:
+            continue
+        stat[info["category_id"]].fp += 1
+
+
 class VpqEvaluator:
     """Feed the sampled frames of one video in order (`add_frame`), then `compute(nframes)` for every window length."""
 
@@ -105,22 +168,7 @@ class VpqEvaluator:
     def add_frame_table(self, gt_segments, pred_segments, pairs, counts):
         """host part of add_frame: (pairs, counts) = the frame's sorted (gt * 2^24 + pred) codes and their pixel counts"""
         gt_segms, pred_segms = _merge_segments(gt_segments), _merge_segments(pred_segments)
-        # predicted areas are recounted from the id map + sanity checks (eval_vpq.py:102-116)
-        area = defaultdict(int)
-        for lab, c in zip((pairs % np.uint64(OFFSET)).tolist(), counts.tolist()):
-            area[lab] += c
-        left = set(el["id"] for el in pred_segments)
-        for lab in sorted(area):
-            if lab not in pred_segms:
-                if lab == VOID:
-                    continue
-                raise KeyError("Segment with ID {} is presented in PNG and not presented in JSON.".format(lab))
-            pred_segms[lab]["area"] = area[lab]
-            left.remove(lab)
-            if pred_segms[lab]["category_id"] not in self.categories:
-                raise KeyError("Segment with ID {} has unknown category_id {}.".format(lab, pred_segms[lab]["category_id"]))
-        if left:
-            raise KeyError("The following segment IDs {} are presented in JSON and not presented in PNG.".format(sorted(left)))
+        recount_pred_areas(pred_segms, pred_segments, pairs, counts, self.categories)
         self.frames.append((gt_segms, pred_segms, pairs, counts))
 
     @staticmethod
@@ -146,38 +194,7 @@ class VpqEvaluator:
                 for lab, c in zip(pairs.tolist(), counts.tolist()):
                     conf[lab] += c
             gt_pred = {(lab // OFFSET, lab % OFFSET): conf[lab] for lab in sorted(conf)}     # np.unique order
-            gt_matched, pred_matched = set(), set()
-            for (g, p), inter in gt_pred.items():                                              # :157-181
-                if g not in vid_gt or p not in vid_pred:
-                    continue
-                if vid_gt[g]["iscrowd"] == 1 or vid_gt[g]["category_id"] != vid_pred[p]["category_id"]:
-                    continue
-                union = vid_pred[p]["area"] + vid_gt[g]["area"] - inter - gt_pred.get((VOID, p), 0)
-                iou = inter / union
-                assert iou <= 1.0, "INVALID IOU VALUE : %d" % g
-                if iou > 0.5:
-                    c = stat[vid_gt[g]["category_id"]]
-                    c.tp += 1
-                    c.iou += iou
-                    gt_matched.add(g)
-                    pred_matched.add(p)
-            crowd = {}
-            for g, info in vid_gt.items():                                                     # :183-192
-                if g in gt_matched:
-                    continue
-                if info["iscrowd"] == 1:
-                    crowd[info["category_id"]] = g
-                    continue
-                stat[info["category_id"]].fn += 1
-            for p, info in vid_pred.items():                                                   # :194-207
-                if p in pred_matched:
-                    continue
-                inter = gt_pred.get((VOID, p), 0)
-                if info["category_id"] in crowd:
-                    inter += gt_pred.get((crowd[info["category_id"]], p), 0)
-                if inter / info["area"] > 0.5:
-                    continue
-                stat[info["category_id"]].fp += 1
+            match_segments(stat, vid_gt, vid_pred, gt_pred, check_iou=True)
         return stat
 
 
