@@ -413,12 +413,27 @@ int vps_pan2ch_image_ids(const uint8_t* pan_2ch, int64_t npix, int num_stuff, ui
 int vps_seg_confusion(const uint8_t* gt, const void* pred, int label_bytes, int64_t npix, int num_classes, uint64_t* conf,
                       void* stream);
 
+/* vps_seg_confusion for a prediction of another shape (ph x pw) than the gt (gh x gw): evaluate_ssegs resizes the prediction
+ * PNG to the gt with Image.NEAREST (tools/dataset/cityscapes.py:125-126), so gt pixel (y, x) is counted against the prediction
+ * at (ytab[y], xtab[x]) (an index < 0 reads 0, Pillow's fill value).  xtab [gw] / ytab [gh]: device int32 index tables of
+ * Pillow's affine scaler (a sequential double sum, built on the host once per shape pair).  pred: uint8 (pred_elem 1) or int64
+ * (pred_elem 8, low byte used); same per-pixel rule as vps_seg_confusion; no resized map is written. */
+int vps_seg_confusion_nearest(const uint8_t* gt, int gh, int gw, const void* pred, int pred_elem, int ph, int pw,
+                              const int* xtab, const int* ytab, int num_classes, uint64_t* conf, void* stream);
+
 /* ---- input stage (SURVEY 8f rank 4) -----------------------------------------------------------------------------------------
  * Normalize (mmcv.imnormalize: float32, BGR->RGB, (x - mean) / std; transforms.py:295-318) + Pad(size_divisor) (zero pad bottom /
  * right, :238-270) + ImageToTensor (HWC -> CHW, formating.py:46-68) of one uint8 HWC BGR frame in one pass: out is fp32 NCHW
  * [1,3,hp,wp].  mean3 / std3 are HOST arrays in output-channel order (RGB when to_rgb).  Bit-identical to the numpy arithmetic. */
 int vps_preprocess_u8(const uint8_t* bgr_hwc, int h, int w, const float* mean3, const float* std3, int to_rgb,
                       float* out_nchw, int hp, int wp, void* stream);
+
+/* Resize(img_scale, keep_ratio=True) in front of the same pass (transforms.py:107-121: mmcv.imrescale -> cv2.resize(...,
+ * INTER_LINEAR) of the uint8 frame, for img and ref_img): the h x w frame is resized to oh x ow with OpenCV's fixed-point
+ * bilinear arithmetic for uint8, bit for bit, then normalised and zero-padded to hp x wp.  Taps are computed on the device
+ * (no host table, capturable); bgr_hwc may have any alignment.  oh == h and ow == w gives vps_preprocess_u8's output. */
+int vps_preprocess_resize_u8(const uint8_t* bgr_hwc, int h, int w, int oh, int ow, const float* mean3, const float* std3,
+                             int to_rgb, float* out_nchw, int hp, int wp, void* stream);
 
 #ifdef __cplusplus
 }

@@ -72,12 +72,12 @@ EXPORTS = [
     "vps_conv2d_tc32", "vps_conv2d_tc32_multi", "vps_conv2d_tc32_plan", "vps_pack_weights_tc32", "vps_packed_tc32_bytes", "vps_tc32_overflow", "vps_deform_conv_tc32", "vps_deform_conv_tc32_plan",
     "vps_correlation", "vps_correlation_tc", "vps_correlation_simt", "vps_correlation_tc32", "vps_correlation_tc32_ws_bytes", "vps_resample2d", "vps_channelnorm", "vps_flownet_input", "vps_flownet_stage", "vps_flownet_cat3", "vps_flow_deconv",
     "vps_nchw_to_nhwc", "vps_nhwc_to_nchw", "vps_copy_scale", "vps_axpby",
-    "vps_space_to_depth2", "vps_tap_gather3x3", "vps_preprocess_u8", "vps_resize_bilinear", "vps_resize_nearest", "vps_pool2d", "vps_groupnorm",
+    "vps_space_to_depth2", "vps_tap_gather3x3", "vps_preprocess_u8", "vps_preprocess_resize_u8", "vps_resize_bilinear", "vps_resize_nearest", "vps_pool2d", "vps_groupnorm",
     "vps_bfp_gather", "vps_bfp_scatter", "vps_flow_warp", "vps_tcea_temporal", "vps_tcea_combine",
     "vps_deform_im2col", "vps_deform_conv_tc",
     "vps_roi_align", "vps_sort_desc", "vps_rpn_decode", "vps_nms", "vps_nms_batch", "vps_sigmoid_flat", "vps_gather_rows",
     "vps_maskroi_candidates", "vps_track_assign",
     "vps_rpn_finalize", "vps_maskroi_finalize", "vps_select_class", "vps_track_update", "vps_det_split",
     "vps_mask_removal", "vps_panoptic_fuse", "vps_unify_pan", "vps_unify_pan_image", "vps_unify_pan_ws_bytes", "vps_unify_pan_error", "vps_unify_pan_error_offset", "vps_tube_confusion", "vps_tube_confusion_ws_bytes", "vps_rgb_to_id", "vps_pan2ch_ids",
-    "vps_pan2ch_image_ids", "vps_seg_confusion",
+    "vps_pan2ch_image_ids", "vps_seg_confusion", "vps_seg_confusion_nearest",
 ]

@@ -26,16 +26,24 @@ __device__ __forceinline__ void load_strip(const TL* __restrict__ p, int64_t i0,
   }
 }
 
-// grid-stride walk over the 16-pixel strips of two maps of npix pixels; flush(a, b, n) once per run of n equal pairs
-template <typename TA, typename TB, typename F>
-__device__ __forceinline__ void walk_label_runs(const TA* __restrict__ a, const TB* __restrict__ b, int64_t npix, F&& flush) {
+// a label map read in place: fetch(i0, cnt, v) fills the strip starting at pixel i0
+template <typename TL>
+struct StripOf {
+  const TL* __restrict__ p;
+  __device__ __forceinline__ void operator()(int64_t i0, int cnt, int (&v)[LABEL_RUN]) const { load_strip(p, i0, cnt, v); }
+};
+
+// grid-stride walk over the 16-pixel strips of two label sources of npix pixels; fetch_a / fetch_b(i0, cnt, v) give each
+// strip's labels (-1 past the end), flush(a, b, n) is called once per run of n equal pairs
+template <typename FA, typename FB, typename F>
+__device__ __forceinline__ void walk_label_runs_by(FA&& fetch_a, FB&& fetch_b, int64_t npix, F&& flush) {
   const int64_t nrun = (npix + LABEL_RUN - 1) / LABEL_RUN;
   VPS_GRID_STRIDE(r, nrun) {
     const int64_t i0 = r * LABEL_RUN;
     const int cnt = (int)min((int64_t)LABEL_RUN, npix - i0);
     int av[LABEL_RUN], bv[LABEL_RUN];
-    load_strip(a, i0, cnt, av);
-    load_strip(b, i0, cnt, bv);
+    fetch_a(i0, cnt, av);
+    fetch_b(i0, cnt, bv);
     int ca = av[0], cb = bv[0];
     unsigned int n = 1;
 #pragma unroll
@@ -46,6 +54,12 @@ __device__ __forceinline__ void walk_label_runs(const TA* __restrict__ a, const 
     }
     flush(ca, cb, n);
   }
+}
+
+// the same walk over two maps stored in place
+template <typename TA, typename TB, typename F>
+__device__ __forceinline__ void walk_label_runs(const TA* __restrict__ a, const TB* __restrict__ b, int64_t npix, F&& flush) {
+  walk_label_runs_by(StripOf<TA>{a}, StripOf<TB>{b}, npix, flush);
 }
 
 }  // namespace vps

@@ -528,6 +528,77 @@ extern "C" int vps_preprocess_u8(const uint8_t* bgr_hwc, int h, int w, const flo
   return VPS_OK;
 }
 
+// Resize(img_scale, keep_ratio) of the same pipeline (transforms.py:107-121: mmcv.imrescale -> cv2.resize(..., INTER_LINEAR)
+// on the uint8 frame) fused in front of Normalize + Pad + ImageToTensor.  OpenCV's fixed-point bilinear path for uint8,
+// bit for bit; the taps are computed here, so there is no per-shape host table or upload and the stage stays capturable:
+//   per axis: scale = 1 / (dst / src) (double); f = (float)((d + 0.5) * scale - 0.5); s = floor(f); f -= s (float);
+//   x: f = 0 where s < 0 (s = 0) or s >= src - 1 (s = src - 1), second tap min(s + 1, src - 1);
+//   y: f kept, both rows clamped to [0, src - 1];   a1 = rint(f * 2048), a0 = rint((1 - f) * 2048) (half to even);
+//   R = S[s0] * a0 + S[s1] * a1 per row; out = clamp((((R0 >> 4) * b0 >> 16) + ((R1 >> 4) * b1 >> 16) + 2) >> 2, 0, 255)
+// (the vertical arithmetic of OpenCV's SIMD VResizeLinearVec_32s8u, which cv2 uses for every column).  Explicitly rounded
+// double operations keep nvcc from contracting (d + 0.5) * scale - 0.5 into an FMA, which would change f.
+namespace {
+struct LinearTap {
+  int s0, s1, a0, a1;
+};
+__device__ __forceinline__ LinearTap linear_tap(int d, int src, double scale, bool clamp_frac) {
+  float f = __double2float_rn(__dadd_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), -0.5));
+  int s = (int)floorf(f);
+  f = __fsub_rn(f, (float)s);
+  if (clamp_frac) {
+    if (s < 0) { f = 0.f; s = 0; }
+    if (s >= src - 1) { f = 0.f; s = src - 1; }
+  }
+  LinearTap t;
+  t.s0 = min(max(s, 0), src - 1);
+  t.s1 = min(max(s + 1, 0), src - 1);
+  t.a1 = __float2int_rn(__fmul_rn(f, 2048.f));
+  t.a0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f));
+  return t;
+}
+
+// grid (cdiv(wp, 256), hp): one thread per output pixel of the padded tensor; source bytes are read one at a time, so any
+// alignment of the frame works (neighbouring threads share most of their taps, which L1 serves)
+__global__ void preprocess_resize_u8_kernel(const uint8_t* __restrict__ src, int h, int w, int oh, int ow, double sy, double sx,
+                                            float m0, float m1, float m2, float s0, float s1, float s2, int to_rgb,
+                                            float* __restrict__ out, int hp, int wp) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+  if (x >= wp) return;
+  float v0 = 0.f, v1 = 0.f, v2 = 0.f;                     // pad_val = 0 after normalisation
+  if (y < oh && x < ow) {
+    const LinearTap tx = linear_tap(x, w, sx, true), ty = linear_tap(y, h, sy, false);
+    const uint8_t* r0 = src + (int64_t)ty.s0 * w * 3;
+    const uint8_t* r1 = src + (int64_t)ty.s1 * w * 3;
+    float c[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const int R0 = (int)r0[tx.s0 * 3 + k] * tx.a0 + (int)r0[tx.s1 * 3 + k] * tx.a1;
+      const int R1 = (int)r1[tx.s0 * 3 + k] * tx.a0 + (int)r1[tx.s1 * 3 + k] * tx.a1;
+      const int t = (((R0 >> 4) * ty.a0) >> 16) + (((R1 >> 4) * ty.a1) >> 16);
+      c[k] = (float)min(max((t + 2) >> 2, 0), 255);
+    }
+    const float c0 = to_rgb ? c[2] : c[0], c2 = to_rgb ? c[0] : c[2];
+    v0 = __fdiv_rn(__fsub_rn(c0, m0), s0);
+    v1 = __fdiv_rn(__fsub_rn(c[1], m1), s1);
+    v2 = __fdiv_rn(__fsub_rn(c2, m2), s2);
+  }
+  const int64_t plane = (int64_t)hp * wp, o = (int64_t)y * wp + x;
+  out[o] = v0; out[plane + o] = v1; out[2 * plane + o] = v2;
+}
+}  // namespace
+
+extern "C" int vps_preprocess_resize_u8(const uint8_t* bgr_hwc, int h, int w, int oh, int ow, const float* mean3,
+                                        const float* std3, int to_rgb, float* out_nchw, int hp, int wp, void* stream) {
+  VPS_CHECK_ARG(h > 0 && w > 0 && oh > 0 && ow > 0 && hp >= oh && wp >= ow, "preprocess_resize_u8: shapes %dx%d -> %dx%d -> %dx%d",
+                h, w, oh, ow, hp, wp);
+  const double sy = 1.0 / ((double)oh / (double)h), sx = 1.0 / ((double)ow / (double)w);     // cv2: scale = 1 / inv_scale
+  dim3 grid((unsigned)((wp + 255) / 256), (unsigned)hp);
+  preprocess_resize_u8_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(bgr_hwc, h, w, oh, ow, sy, sx, mean3[0], mean3[1], mean3[2],
+                                                                     std3[0], std3[1], std3[2], to_rgb, out_nchw, hp, wp);
+  VPS_CUDA_LAST("preprocess_resize_u8");
+  return VPS_OK;
+}
+
 // ---------------------------------------------------------------- 3x3 convolutions with <= 3 output channels (predict_flow)
 // FlowNet2's predict_flow layers (submodules.py:27-28: Conv2d(cin, 2, 3, 1, 1), 19 launches per pair) have K = 9*cin up to
 // 9234 but N = 2: as implicit GEMMs they cost one K step per (tap, 32 channels) at any N.  They run as a 1x1 tensor-core

@@ -2,8 +2,9 @@
 passes on the GPU:
 
 * semantic mIoU -- `Cityscapes.evaluate_ssegs` (tools/dataset/cityscapes.py:112-166): a C x C confusion matrix of gt
-  trainIds against `fcn_outputs`, accumulated over frames on the device (`vps_seg_confusion`); applies to every model's
-  `fcn_outputs`;
+  trainIds against `fcn_outputs`, accumulated over frames on the device (`vps_seg_confusion`; with `resize_pred`, a
+  prediction of another shape is read through the reference's Image.NEAREST resize, `vps_seg_confusion_nearest`); applies
+  to every model's `fcn_outputs`;
 * image PQ -- `BaseDataset.evaluate_panoptic` (tools/dataset/base_dataset.py:104-229): the image converter's segment keying
   (`vps_pan2ch_image_ids`), the frame's (gt, pred) pair table (`vps_tube_confusion`, whose row sums are the predicted
   areas), then `_pq_compute_single_core` (:337-431) on the host in the reference's order, so the IoU sums are identical,
@@ -19,31 +20,60 @@ from ._lib import lib
 from .vpq import OFFSET, VOID, CatStat, frame_confusion, match_segments, pq_average, recount_pred_areas, rgb_to_id
 
 
+def nearest_table(src, dst):
+    """Pillow's index table of one axis of Image.resize(size, NEAREST) (the affine scaler of a pure scale): a = src / dst,
+    xo = a / 2, then per output index int(xo) and xo += a.  The sum is sequential in double, so it is built here, once,
+    rather than on the device; -1 marks an index outside the source (the pixel then reads Pillow's fill value 0)."""
+    if src == dst:
+        return np.arange(dst, dtype=np.int32)                     # Pillow copies an image whose size is unchanged
+    a = float(src) / float(dst)
+    xo = np.cumsum(np.concatenate([[a * 0.5], np.full(dst - 1, a)]))
+    idx = np.where(xo < 0, -1, xo.astype(np.int64))
+    return np.where((idx >= 0) & (idx < src), idx, -1).astype(np.int32)
+
+
 class SegEvaluator:
     """Semantic mIoU of `Cityscapes.evaluate_ssegs`: `add_frame` per frame, `result()` once."""
 
-    def __init__(self, num_classes=19):
+    def __init__(self, num_classes=19, resize_pred=False):
         self.num_classes = num_classes
+        # resize_pred: a prediction of another shape than the gt is resized to it with Image.NEAREST, as evaluate_ssegs does
+        # with the PNG it wrote (cityscapes.py:125-126); the index tables are device arrays cached per (pred, gt) shape
+        self.resize_pred = bool(resize_pred)
+        self._tables = {}
         self._conf = None               # device uint64 [C, C] (held as int64), row = gt
+
+    def _nearest_tables(self, ph, pw, gh, gw, device):
+        key = (ph, pw, gh, gw, device)
+        if key not in self._tables:
+            self._tables[key] = tuple(torch.from_numpy(nearest_table(s, d)).to(device) for s, d in ((pw, gw), (ph, gh)))
+        return self._tables[key]
 
     @torch.no_grad()
     def add_frame(self, gt_trainids, fcn_output):
         """gt_trainids: uint8 CUDA map; fcn_output: uint8 or int64 CUDA map of the same [H,W] (a leading 1 is allowed).
-        The reference resizes the prediction to the gt with Image.NEAREST, which is the identity only for equal shapes:
-        other shapes raise."""
+        The reference resizes the prediction to the gt with Image.NEAREST, which is the identity for equal shapes.  Other
+        shapes raise unless the evaluator was made with resize_pred=True, which applies that resize."""
         if not (gt_trainids.is_cuda and fcn_output.is_cuda):
             raise RuntimeError("SegEvaluator: label maps must be CUDA tensors (there is no CPU path)")
         if gt_trainids.dtype != torch.uint8 or fcn_output.dtype not in (torch.uint8, torch.int64):
             raise TypeError("SegEvaluator: gt must be uint8 and the prediction uint8 or int64")
         g, p = gt_trainids.squeeze(0), fcn_output.squeeze(0)
-        if g.dim() != 2 or g.shape != p.shape:
+        if g.dim() != 2 or p.dim() != 2 or (g.shape != p.shape and not self.resize_pred):
             raise ValueError("SegEvaluator: gt %s and prediction %s must be [H,W] maps of the same shape"
                              % (tuple(gt_trainids.shape), tuple(fcn_output.shape)))
         g, p = g.contiguous(), p.contiguous()
         if self._conf is None:
             self._conf = torch.zeros(self.num_classes, self.num_classes, dtype=torch.int64, device=g.device)
-        ops.check(lib().vps_seg_confusion(ops._ptr(g), ops._ptr(p), p.element_size(), C.c_int64(g.numel()), self.num_classes,
-                                          ops._ptr(self._conf), ops.stream()), "seg_confusion")
+        if g.shape == p.shape:
+            ops.check(lib().vps_seg_confusion(ops._ptr(g), ops._ptr(p), p.element_size(), C.c_int64(g.numel()), self.num_classes,
+                                              ops._ptr(self._conf), ops.stream()), "seg_confusion")
+            return
+        (gh, gw), (ph, pw) = g.shape, p.shape
+        xtab, ytab = self._nearest_tables(ph, pw, gh, gw, g.device)
+        ops.check(lib().vps_seg_confusion_nearest(ops._ptr(g), gh, gw, ops._ptr(p), p.element_size(), ph, pw, ops._ptr(xtab),
+                                                  ops._ptr(ytab), self.num_classes, ops._ptr(self._conf), ops.stream()),
+                  "seg_confusion_nearest")
 
     def confusion_matrix(self):
         """the accumulated counts, float64 [C, C] as the reference holds them"""
@@ -81,7 +111,8 @@ class IpqEvaluator:
 
     def add_frame(self, gt_rgb, gt_segments, pan_2ch):
         """gt_rgb: RGB panoptic ground truth (uint8 CUDA [H,W,3]) with its segments_info list; pan_2ch: the image-level
-        unified result (uint8 CUDA [H,W,3]) of the same size.  The predicted segments are the converter's: category =
+        unified result (uint8 CUDA [H,W,3]) of the same size.  Other sizes raise, and there is no resizing mode: the
+        reference's PQ core compares the PNGs pixel for pixel and fails on maps of different sizes too.  The predicted segments are the converter's: category =
         semantic class, iscrowd 0, area = pixel count (the row sums of the frame's pair table)."""
         if gt_rgb.shape != pan_2ch.shape:
             raise ValueError("IpqEvaluator: gt %s and prediction %s differ in shape" % (tuple(gt_rgb.shape), tuple(pan_2ch.shape)))

@@ -18,13 +18,16 @@ reference frame is uploaded or normalised.  PanopticFuse has no tracker: with `u
 result (`PanUnifier(image=True)`)."""
 import torch
 
+from .pipeline import GEOMETRY_KEYS
+
 
 class ClipRunner:
     def __init__(self, det, device=None, depth=2, unify=False, streaming=False, input_stage=None):
         self.det = det
         # input_stage: a vps_b200.pipeline.InputStage -- the pairs are then decoded uint8 HWC BGR frames (what the reference's
         # loader produces before Normalize / Pad / ImageToTensor); they are uploaded as uint8 (4x fewer bytes) and normalised,
-        # padded and transposed on the device
+        # padded and transposed on the device; a stage with resize=True also resizes them, and its geometry fields replace the
+        # caller's in the meta handed to the detector
         self.input_stage = input_stage
         self._f32, self._nf32 = [], 0
         # streaming: every pair's reference frame is the previous pair's current frame (the clip chain of
@@ -92,22 +95,23 @@ class ClipRunner:
         if self.streaming:
             self._prev_feats = self.det._pf_queue[-1][2]['x'] if self.det._pf_queue else None
 
-    def _normalise(self, staged):
-        """uint8 HWC device frames -> fp32 NCHW padded tensors (ring of 3 like the upload ring)"""
+    def _normalise(self, staged, meta):
+        """uint8 HWC device frames -> fp32 NCHW padded tensors (ring of 3 like the upload ring) and the pair's meta: when the
+        stage resizes, its ori_shape / img_shape / pad_shape / scale_factor replace the caller's (filename / iid stay)"""
         slot = self._nf32 % 3
         self._nf32 += 1
         while len(self._f32) <= slot:
             self._f32.append([None, None])
-        outs = []
-        for k in (0, 1):
-            if staged[k] is None:
-                outs.append(None)
-                continue
-            o, _ = self.input_stage(staged[k], out=self._f32[slot][k] if (self._f32[slot][k] is not None and
-                                                                            self._f32[slot][k].shape[2] >= staged[k].shape[0]) else None)
-            self._f32[slot][k] = o
-            outs.append(o)
-        return outs[0], outs[1], None
+        ring = self._f32[slot]
+        for k in (0, 1):                            # a buffer is reused only for the output shape it was made for
+            if ring[k] is not None and (staged[k] is None or tuple(ring[k].shape[2:]) !=
+                                        self.input_stage.geometry(int(staged[k].shape[0]), int(staged[k].shape[1]))[2:4]):
+                ring[k] = None
+        a, b, m = self.input_stage.pair(staged[0], staged[1], outs=ring)
+        ring[0], ring[1] = a, b
+        if self.input_stage.resize:
+            meta = dict(meta, **{k: m[k] for k in GEOMETRY_KEYS})
+        return (a, b, None), meta
 
     def _stage(self, pair, resident):
         """make the pair available on the device: (img, ref, event or None)"""
@@ -133,7 +137,8 @@ class ClipRunner:
         if staged[2] is not None:
             main.wait_event(staged[2])
         if self.input_stage is not None:
-            staged = self._normalise(staged)
+            staged, m = self._normalise(staged, cur[1])
+            cur = (cur[0], m)
         self._prev_feats = None
         self._chain = []        # streaming: static-part outputs of enqueued pairs, in order (their 'x' feeds the next pair)
         if prefetch:
@@ -149,7 +154,8 @@ class ClipRunner:
                 if staged[2] is not None:
                     main.wait_event(staged[2])
                 if self.input_stage is not None:
-                    staged = self._normalise(staged)
+                    staged, m = self._normalise(staged, cur[1])
+                    cur = (cur[0], m)
                 if prefetch:
                     self._prefetch(staged, cur[1])
             rb = [b] if b is not None else None

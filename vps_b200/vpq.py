@@ -161,7 +161,8 @@ class VpqEvaluator:
         self.frames = []            # (gt_segms, pred_segms, pairs, counts)
 
     def add_frame(self, gt_segments, pred_segments, gt_ids, pred_ids):
-        """gt_ids / pred_ids: CUDA id maps of one sampled frame"""
+        """gt_ids / pred_ids: CUDA id maps of one sampled frame, of one size.  There is no resizing mode: the reference's VPQ
+        core compares the PNGs pixel for pixel and fails on maps of different sizes too."""
         pairs, counts = frame_confusion(gt_ids, pred_ids)
         self.add_frame_table(gt_segments, pred_segments, pairs, counts)
 
