@@ -405,6 +405,25 @@ int vps_pan2ch_ids(const uint8_t* pan_2ch, int64_t npix, int num_stuff, uint32_t
  * VOID -> 0 */
 int vps_pan2ch_image_ids(const uint8_t* pan_2ch, int64_t npix, int num_stuff, uint32_t* ids, void* stream);
 
+/* ---- segment table of the video writer (converter_2ch_track_core, tools/dataset/cityscapes_vps.py:96-140) -------------
+ * One pass over a unified 3-channel result pan_2ch [H,W,3] (device uint8, channel 0 semantic, channel 2 track).  Keys are
+ * (semantic < VPS_SEG_NSEM, track byte), key = 256 * semantic + track; VOID (semantic 255) is skipped.  table (device
+ * uint32 [VPS_SEG_TABLE_WORDS], overwritten) holds VPS_SEG_PLANES planes of VPS_SEG_NKEY words -- pixel count, min x,
+ * min y, max x, max y per key (an untouched key keeps count 0, min 0xFFFFFFFF, max 0) -- and one last word counting
+ * pixels whose semantic is neither < VPS_SEG_NSEM nor 255.  rgb_out (device uint8 [H,W,3], or NULL) receives id2rgb of the
+ * segment id: 1000 * semantic + 1 for semantic < num_stuff, 1000 * semantic + track + 1 otherwise, 0 for VOID and for
+ * the invalid semantics. */
+#define VPS_SEG_NSEM 19
+#define VPS_SEG_NKEY (VPS_SEG_NSEM * 256)
+#define VPS_SEG_PLANES 5
+#define VPS_SEG_AREA 0
+#define VPS_SEG_X0 1
+#define VPS_SEG_Y0 2
+#define VPS_SEG_X1 3
+#define VPS_SEG_Y1 4
+#define VPS_SEG_TABLE_WORDS (VPS_SEG_PLANES * VPS_SEG_NKEY + 1)
+int vps_pan2ch_segments(const uint8_t* pan_2ch, int H, int W, int num_stuff, uint32_t* table, uint8_t* rgb_out, void* stream);
+
 /* ---- semantic mIoU of the reference (Cityscapes.evaluate_ssegs, tools/dataset/cityscapes.py:112-166) ----------------
  * ADDS the confusion counts of one frame into conf (device uint64 [num_classes * num_classes], row = gt): index
  * gt * C + pred over the pixels with gt != 255, counted iff index < C * C (np.bincount + the reference's copy loop,

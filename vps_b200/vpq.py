@@ -218,3 +218,75 @@ def pq_average(stat, categories, isthing=None):
         per_class[label] = {"pq": pq_c, "sq": sq_c, "rq": rq_c, "iou": c.iou, "tp": c.tp, "fp": c.fp, "fn": c.fn}
         pq += pq_c; sq += sq_c; rq += rq_c
     return {"pq": pq / n, "sq": sq / n, "rq": rq / n, "n": n}, per_class
+
+
+NFRAMES_PER_VIDEO = 6           # eval_vpq.py:305: the GT frames of one clip
+WINDOWS = (1, 2, 3, 4)          # nframes of the tubes, k = 5 * (nframes - 1) = 0, 5, 10, 15
+
+
+def split_clips(n_frames, n_annotations, nframes_per_video=NFRAMES_PER_VIDEO):
+    """frame indices of each clip: np.array_split of the split's frames into len(gt annotations) // 6 clips (eval_vpq.py:306-309;
+    the sizes differ by at most one when the count is uneven)"""
+    return [c.tolist() for c in np.array_split(np.arange(n_frames), n_annotations // nframes_per_video)]
+
+
+def _id_map(img):
+    """RGB-coded id image (numpy or torch, [H,W,>=3] uint8) -> int32 CUDA id map"""
+    t = img if torch.is_tensor(img) else torch.from_numpy(np.ascontiguousarray(img))
+    if t.dim() != 3 or t.shape[2] < 3 or t.dtype != torch.uint8:
+        raise ValueError("id image must be uint8 [H, W, 3], got %s %s" % (tuple(t.shape), t.dtype))
+    return rgb_to_id(t[..., :3].to("cuda", non_blocking=True).contiguous())
+
+
+def evaluate_split(gt_json, pred_json, gt_maps, pred_maps, nframes_per_video=NFRAMES_PER_VIDEO, windows=WINDOWS):
+    """VPQ of a whole split as tools/eval_vpq.py's main computes it (:281-323), without the files: gt_json / pred_json are
+    the loaded JSONs, gt_maps / pred_maps iterables of RGB-coded id images (host or CUDA uint8 [H,W,3]) in the order the
+    reference pairs them with the annotations -- zip(gt annotations, pred annotations, gt maps, pred maps).  The maps are
+    consumed one frame at a time: each frame's (gt, pred) pair table is built once on the device and the images are dropped.
+    Returns {k: {"All", "Things", "Stuff": pq_average results, "per_class": per-category results}} for k = 5 * (nframes - 1).
+    Each clip's statistics are summed into the split's in clip order, as PQStat.__iadd__ does, so the IoU sums are the
+    reference's to the bit."""
+    categories = {el["id"]: el for el in gt_json["categories"]}
+    gt_anns, pred_anns = gt_json["annotations"], pred_json["annotations"]
+    tables = []
+    for (g, p), _ in zip(zip(gt_maps, pred_maps), range(min(len(gt_anns), len(pred_anns)))):
+        tables.append(frame_confusion(_id_map(g), _id_map(p)))
+    stats = {nf: defaultdict(CatStat) for nf in windows}
+    for clip in split_clips(len(tables), len(gt_anns), nframes_per_video):
+        ev = VpqEvaluator(categories)
+        for i in clip:
+            ev.add_frame_table(gt_anns[i]["segments_info"], pred_anns[i]["segments_info"], *tables[i])
+        for nf in windows:
+            for c, v in ev.compute(nf).items():
+                stats[nf][c] += v
+    out = {}
+    for nf in windows:
+        res = {}
+        for name, isthing in (("All", None), ("Things", True), ("Stuff", False)):
+            res[name], per_class = pq_average(stats[nf], categories, isthing=isthing)
+            if name == "All":
+                res["per_class"] = per_class
+        out[5 * (nf - 1)] = res
+    return out
+
+
+def vpq_text(res):
+    """the text of vpq-<k>.txt (eval_vpq.py:233-244) for one entry of evaluate_split's result"""
+    lines = ["================================================\n",
+             "{:10s}| {:>5s}  {:>5s}  {:>5s} {:>5s}".format("", "PQ", "SQ", "RQ", "N\n"),
+             "-" * 38 + "\n"]
+    for name in ("All", "Things", "Stuff"):
+        r = res[name]
+        lines.append("{:10s}| {:5.1f}  {:5.1f}  {:5.1f} {:5d}\n".format(name, 100 * r["pq"], 100 * r["sq"], 100 * r["rq"], r["n"]))
+    lines.append("{:4s}| {:>5s} {:>5s} {:>5s} {:>6s} {:>7s} {:>7s} {:>7s}\n".format("IDX", "PQ", "SQ", "RQ", "IoU", "TP", "FP", "FN"))
+    for idx, r in res["per_class"].items():
+        lines.append("{:4d} | {:5.1f} {:5.1f} {:5.1f} {:6.1f} {:7d} {:7d} {:7d}\n".format(
+            idx, 100 * r["pq"], 100 * r["sq"], 100 * r["rq"], r["iou"], r["tp"], r["fp"], r["fn"]))
+    return "".join(lines)
+
+
+def vpq_final_text(results):
+    """the text of vpq-final.txt (eval_vpq.py:325-330): the mean over k of 100 * PQ for All, Things and Stuff"""
+    ks = sorted(results)
+    mean = lambda name: sum(100 * results[k][name]["pq"] for k in ks) / len(ks)
+    return "vpq_all:%.4f\nvpq_thing:%.4f\nvpq_stuff:%.4f\n" % (mean("All"), mean("Things"), mean("Stuff"))

@@ -1,17 +1,24 @@
 """2-channel -> PNG / JSON writer (SURVEY 8f rank 1b): `converter_2ch_track_core` + the file layout of
 `inference_panoptic_video` (reference tools/dataset/cityscapes_vps.py:26-160), frame by frame.
 
-The device part is two tested ops -- `vps_pan2ch_ids` (segment key per pixel) and the sort + run-length table of
-`vps_tube_confusion` (segment areas), both through `vps_b200.vpq.segments_from_pan2ch`; bounding boxes, PNG encoding and the
-JSON are host work (they end in files).  Segment ids: the reference uses the colours of panopticapi's `IdGenerator` (one fixed
+`PanWriter.add_frame` makes one device pass per sampled frame (`vps_pan2ch_segments`): the pixel count and bounding box of
+every (semantic, track) key and the pan_pred image, id2rgb of the segment id.  The host turns the 19 x 256 key table into
+segments_info (`segments_from_table`) and hands the two PNGs to a small pool of writer threads, so their encoding overlaps
+the next frames; `finish()` waits for them.  `add_frame_ids` is the same host part fed from numpy (scipy find_objects).  Segment ids: the reference uses the colours of panopticapi's `IdGenerator` (one fixed
 colour per stuff category, random per thing key; everything downstream is invariant to the values); here id =
 1000 * semantic + 1 for stuff, 1000 * semantic + track + 1 for things, colour = id2rgb(id).  One reference quirk is kept:
 the bbox of a stuff segment that merges several keys is the bbox of its LAST key (segm_info[colour] is overwritten per key,
 cityscapes_vps.py:131-138) -- `add_frame_ids` takes it from `bbox_ids` when given."""
+import ctypes as C
 import json
 import os
+from collections import deque
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
+
+NSEM, NTRK = 19, 256            # key space of vps_pan2ch_segments (include/vps_b200.h: VPS_SEG_*)
+NKEY = NSEM * NTRK
 
 
 def id2rgb(ids):
@@ -38,30 +45,129 @@ def last_key_ids(pan_2ch, num_stuff=11):
     return out
 
 
+def pan2ch_segments(pan_2ch, num_stuff=11, rgb=True):
+    """The device pass of add_frame: pan_2ch uint8 CUDA [H,W,3] -> (table uint32 numpy [5, 19, 256] of per-key pixel count,
+    min x, min y, max x, max y; pan_pred uint8 CUDA [H,W,3] or None).  Semantics other than 0..18 and 255 raise ValueError."""
+    import torch
+
+    from . import ops
+    from ._lib import lib
+    assert pan_2ch.is_cuda and pan_2ch.dtype == torch.uint8 and pan_2ch.dim() == 3 and pan_2ch.shape[2] == 3
+    p2 = pan_2ch.contiguous()
+    H, W = int(p2.shape[0]), int(p2.shape[1])
+    table = torch.empty(5 * NKEY + 1, dtype=torch.int32, device=p2.device)
+    out = torch.empty_like(p2) if rgb else None
+    ops.check(lib().vps_pan2ch_segments(ops._ptr(p2), H, W, int(num_stuff), ops._ptr(table), ops._ptr(out),
+                                        ops.stream()), "pan2ch_segments")
+    t = table.cpu().numpy().view(np.uint32)
+    if t[-1]:
+        raise ValueError("pan2ch_segments: %d pixels have a semantic class outside 0..%d and 255" % (int(t[-1]), NSEM - 1))
+    return t[:-1].reshape(5, NSEM, NTRK), out
+
+
+def segments_from_table(table, num_stuff=11):
+    """segments_info of one frame from the key table of `pan2ch_segments`, in ascending id order (add_frame_ids' order).
+    A stuff category is one segment: its area is the sum over its keys and its bbox is the bbox of its LARGEST track key
+    (the converter overwrites segm_info[colour] per key in ascending order, `last_key_ids`); a thing key is its own segment."""
+    area, x0, y0, x1, y1 = (table[i] for i in range(5))
+    info = []
+    for sem in range(NSEM):
+        trks = np.flatnonzero(area[sem])
+        if len(trks) == 0:
+            continue
+        if sem < num_stuff:
+            segs = [(1000 * sem + 1, int(area[sem].sum(dtype=np.int64)), int(trks[-1]))]
+        else:
+            segs = [(1000 * sem + int(t) + 1, int(area[sem, t]), int(t)) for t in trks.tolist()]
+        for i, a, t in segs:
+            x, y = int(x0[sem, t]), int(y0[sem, t])
+            info.append({"category_id": sem, "iscrowd": 0, "id": i, "bbox": [x, y, int(x1[sem, t]) - x, int(y1[sem, t]) - y],
+                         "area": a})
+    return info
+
+
+def _save_png(path, img):
+    from PIL import Image
+    os.makedirs(os.path.dirname(path), exist_ok=True)
+    Image.fromarray(img).save(path)
+
+
 class PanWriter:
     """Feed the unified 3-channel results of a clip in order; sampled frames ([(labeled_fid // lambda_)::lambda_], :35) are
-    converted and written to <output_dir>/pan_2ch/ and <output_dir>/pan_pred/; `finish()` writes pred.json."""
+    converted and written to <output_dir>/pan_2ch/ and <output_dir>/pan_pred/; `finish()` writes pred.json.
 
-    def __init__(self, output_dir=None, labeled_fid=20, lambda_=5, sample=True):
+    add_frame encodes its PNGs on `workers` threads with at most `max_pending` frames queued (each holds two host images),
+    so host memory stays bounded; finish() or close() (also on leaving a `with` block) joins them, and a failed write is
+    raised there or by a later add_frame."""
+
+    def __init__(self, output_dir=None, labeled_fid=20, lambda_=5, sample=True, workers=4, max_pending=8):
         self.output_dir = output_dir
         self.start, self.step = (labeled_fid // lambda_, lambda_) if sample else (0, 1)
         self.index = 0
         self.annotations, self.names = [], []
+        self.workers, self.max_pending = max(1, int(workers)), max(1, int(max_pending))
+        self._pool, self._pending = None, deque()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, exc_type, exc, tb):
+        # an exception already on its way out is not replaced by a failed PNG write
+        self.close(raise_errors=exc_type is None)
+        return False
+
+    def _submit(self, name, images):
+        if self._pool is None:
+            self._pool = ThreadPoolExecutor(max_workers=self.workers, thread_name_prefix="pan_writer")
+        while self._pending and len(self._pending) + len(images) > 2 * self.max_pending:
+            self._pending.popleft().result()
+        fn = _clean_name(name)
+        for sub, img in images:
+            self._pending.append(self._pool.submit(_save_png, os.path.join(self.output_dir, sub, fn), img))
+
+    def _drain(self, raise_errors=True):
+        while self._pending:
+            f = self._pending.popleft()
+            if raise_errors:
+                f.result()
+            else:
+                f.exception()                                      # wait for it, keep its error out of the way
+
+    def close(self, raise_errors=True):
+        """wait for the queued PNGs and stop the writer threads (the first failed write is raised unless raise_errors is
+        False)"""
+        try:
+            self._drain(raise_errors)
+        finally:
+            self._pending.clear()
+            if self._pool is not None:
+                self._pool.shutdown(wait=True)
+                self._pool = None
 
     def _sampled(self):
         i = self.index
         self.index += 1
         return i >= self.start and (i - self.start) % self.step == 0
 
-    def add_frame(self, name, pan_2ch):
-        """pan_2ch: uint8 CUDA tensor [H,W,3] (vps_b200.postproc.PanUnifier).  Returns the frame's annotation or None if the
-        frame is not a sampled one."""
+    def add_frame(self, name, pan_2ch, num_stuff=11, pan_2ch_host=None):
+        """pan_2ch: uint8 tensor [H,W,3] (vps_b200.postproc.PanUnifier), on the device (ClipRunner's
+        pano_results['pan_2ch_device']) or on the host (pano_results['pan_2ch']; it is then uploaded).  pan_2ch_host: a host
+        copy of the same image, if the caller has one (pano_results['pan_2ch']): the pan_2ch PNG is encoded from it instead
+        of downloading the device tensor.  Returns the frame's annotation or None if the frame is not a sampled one."""
         if not self._sampled():
             return None
-        from .vpq import segments_from_pan2ch
-        ids, segs = segments_from_pan2ch(pan_2ch)
-        p2 = pan_2ch.cpu().numpy()
-        return self.add_frame_ids(name, ids.cpu().numpy().astype(np.uint32), segs, p2, _counted=True, bbox_ids=last_key_ids(p2))
+        import torch
+        if pan_2ch_host is None and not pan_2ch.is_cuda:
+            pan_2ch_host = pan_2ch
+        dev = pan_2ch if pan_2ch.is_cuda else pan_2ch.to(torch.device("cuda", torch.cuda.current_device()))
+        table, rgb = pan2ch_segments(dev, num_stuff, rgb=self.output_dir is not None)
+        ann = {"segments_info": segments_from_table(table, num_stuff)}
+        self.annotations.append(ann)
+        self.names.append(name)
+        if self.output_dir is not None:
+            p2 = pan_2ch.cpu().numpy() if pan_2ch_host is None else pan_2ch_host.numpy().copy()   # host buffers may be reused
+            self._submit(name, (("pan_pred", rgb.cpu().numpy()), ("pan_2ch", p2)))
+        return ann
 
     def add_frame_ids(self, name, ids, segs, pan_2ch=None, _counted=False, bbox_ids=None):
         """host part: ids [H,W] uint32 (0 = VOID), segs = [{id, category_id, iscrowd, area}] (any order); bbox_ids: id map
@@ -101,6 +207,7 @@ class PanWriter:
         return ann
 
     def finish(self):
+        self.close()
         pred_json = {"annotations": self.annotations}
         if self.output_dir is not None:
             os.makedirs(self.output_dir, exist_ok=True)
