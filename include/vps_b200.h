@@ -358,7 +358,9 @@ int vps_mask_removal(const float* boxes, const int32_t* order, int k, const int*
  * (upsnetFPN.py:59,80) computed in registers; pano_out = argmax over [stuff(num_stuff) | kept
  * instances (seg term + pasted mask logit)], sem_out = argmax over all classes; [H,W] each, stored as int64
  * (label_bytes 8, the dtype torch.max returns in the reference) or uint8 (label_bytes 1, same values, 8x less D2H).
- * dummy != 0: the MaskROI "no detection" result (one all-zero instance channel). */
+ * dummy != 0: the MaskROI "no detection" result (one all-zero instance channel).
+ * *nkeep_dev == 0 (MaskRemoval kept nothing, dummy == 0): one instance, detection 0 in the original order, with its
+ * SegTerm channel and no mask energy, as the reference's keep_inds = [0] fallback (mask_removal.py:89-91). */
 int vps_panoptic_fuse(const vps_tensor* fcn_score, const float* boxes, const int32_t* cls_idx,
                       const float* mask_logit, int msize, const int32_t* keep_sorted, const int* nkeep_dev,
                       int kcap, int num_stuff, int dummy, int H, int W, void* pano_out, void* sem_out,

@@ -188,10 +188,14 @@ __global__ void fuse_prepare_kernel(const float* __restrict__ boxes, const int32
                                     const int32_t* __restrict__ keep_sorted, const int* __restrict__ nkeep_dev, int kcap,
                                     int num_stuff, int H, int W, InstParams* __restrict__ ip, int* __restrict__ ninst) {
   const int j = threadIdx.x;
-  int nk = min(*nkeep_dev, kcap);
+  // MaskRemoval kept nothing: the reference falls back to keep_inds = [0] with an all-zero mask energy
+  // (mask_removal.py:89-91), so detection 0 (original order) still adds its SegTerm channel
+  const int nkeep = *nkeep_dev;
+  const bool fallback = nkeep == 0;
+  const int nk = min(fallback ? 1 : nkeep, kcap);
   if (j == 0) *ninst = nk;
   if (j >= nk) return;
-  const int det = keep_sorted[j];
+  const int det = fallback ? 0 : keep_sorted[j];
   const float* b = boxes + (int64_t)det * 4;
   const int cls = cls_idx[det];
   ip->det[j] = det;
@@ -202,6 +206,7 @@ __global__ void fuse_prepare_kernel(const float* __restrict__ boxes, const int32
   const BoxI r = int_box(b, H, W);
   ip->bx1[j] = r.x1; ip->by1[j] = r.y1; ip->bw[j] = r.w; ip->bh[j] = r.h;
   ip->px0[j] = r.x_0; ip->px1[j] = r.x_1; ip->py0[j] = r.y_0; ip->py1[j] = r.y_1;
+  if (fallback) { ip->px0[j] = ip->px1[j] = ip->py0[j] = ip->py1[j] = 0; }   // empty paste box: no mask energy
 }
 
 // One block = one 32 x 8 pixel tile.  Instances whose SegTerm box and paste box both miss the tile contribute the
