@@ -425,6 +425,14 @@ int vps_pan2ch_image_ids(const uint8_t* pan_2ch, int64_t npix, int num_stuff, ui
 #define VPS_SEG_Y1 4
 #define VPS_SEG_TABLE_WORDS (VPS_SEG_PLANES * VPS_SEG_NKEY + 1)
 int vps_pan2ch_segments(const uint8_t* pan_2ch, int H, int W, int num_stuff, uint32_t* table, uint8_t* rgb_out, void* stream);
+/* the same table for the image converter _converter_2ch_single_core (tools/dataset/base_dataset.py:287-335), which keys
+ * pixels by 1000 * semantic + instance rank: channel 1 takes the place of the track channel, key = 256 * semantic +
+ * channel 1, VOID skipped, invalid semantics counted in the last word.  rgb_out (or NULL) receives id2rgb of the image
+ * converter's segment id, that of vps_pan2ch_image_ids: 1000 * semantic + 1 for semantic < num_stuff, 1000 * semantic +
+ * instance + 1 otherwise, 0 for VOID and for the invalid semantics.
+ * Python: vps_b200.ops.pan2ch_segments(..., image=True) */
+int vps_pan2ch_image_segments(const uint8_t* pan_2ch, int H, int W, int num_stuff, uint32_t* table, uint8_t* rgb_out,
+                              void* stream);
 
 /* ---- semantic mIoU of the reference (Cityscapes.evaluate_ssegs, tools/dataset/cityscapes.py:112-166) ----------------
  * ADDS the confusion counts of one frame into conf (device uint64 [num_classes * num_classes], row = gt): index

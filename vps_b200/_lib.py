@@ -80,4 +80,5 @@ EXPORTS = [
     "vps_rpn_finalize", "vps_maskroi_finalize", "vps_select_class", "vps_track_update", "vps_det_split",
     "vps_mask_removal", "vps_panoptic_fuse", "vps_unify_pan", "vps_unify_pan_image", "vps_unify_pan_ws_bytes", "vps_unify_pan_error", "vps_unify_pan_error_offset", "vps_tube_confusion", "vps_tube_confusion_ws_bytes", "vps_rgb_to_id", "vps_pan2ch_ids",
     "vps_pan2ch_image_ids", "vps_seg_confusion", "vps_seg_confusion_nearest", "vps_pan2ch_segments",
+    "vps_pan2ch_image_segments",
 ]

@@ -1,8 +1,10 @@
 // Segment table of one sampled frame for the video writer (reference tools/dataset/cityscapes_vps.py:96-140,
 // converter_2ch_track_core): the per-key pixel counts and bounding boxes the converter takes from np.unique / np.where over
 // pan = 1000 * semantic + track, and the pan_pred PNG (id2rgb of the segment id), in one pass over the unified result.
+// The image converter (tools/dataset/base_dataset.py:287-335, _converter_2ch_single_core) does the same over
+// pan = 1000 * semantic + instance rank: KEY_CH selects the key channel, 2 (track) or 1 (instance), as in vpq.cu.
 //
-// Keys are (semantic < 19, track byte): at most 19 * 256 of them, so a block keeps the whole table in shared memory
+// Keys are (semantic < 19, key-channel byte): at most 19 * 256 of them, so a block keeps the whole table in shared memory
 // (5 planes x 4864 words = 95 KiB).  Each thread walks strips of 16 pixels inside one row and issues one set of shared
 // atomics per run of equal keys; a block then adds each key it touched into the global table with one atomic per plane.
 #include "common.cuh"
@@ -21,6 +23,7 @@ __global__ void seg_table_init_kernel(uint32_t* __restrict__ table) {
 }
 
 // vec: W % 16 == 0 and both images 16-byte aligned, so every strip is three aligned uint4 of input and of output
+template <int KEY_CH>
 __global__ void __launch_bounds__(256) pan2ch_segments_kernel(const uint8_t* __restrict__ p2, int H, int W, uint32_t num_stuff,
                                                               uint32_t* __restrict__ table, uint8_t* __restrict__ rgb, bool vec) {
   extern __shared__ uint32_t s[];                                  // planes area, x0, y0, x1, y1 of NKEY words
@@ -62,7 +65,7 @@ __global__ void __launch_bounds__(256) pan2ch_segments_kernel(const uint8_t* __r
 #pragma unroll
     for (int e = 0; e < SEG_RUN; ++e) {
       if (e < cnt) {
-        const uint32_t sem = px[3 * e], trk = px[3 * e + 2];
+        const uint32_t sem = px[3 * e], trk = px[3 * e + KEY_CH];
         const int key = sem == 255u ? -1 : (sem < (uint32_t)VPS_SEG_NSEM ? (int)(sem * 256u + trk) : -2);
         const uint32_t id = key == -2 ? 0u : seg_id(sem, trk, num_stuff);
         out[3 * e] = (uint8_t)(id & 255u);
@@ -100,10 +103,8 @@ __global__ void __launch_bounds__(256) pan2ch_segments_kernel(const uint8_t* __r
   }
   if (threadIdx.x == 0 && s_bad != 0) atomicAdd(&table[VPS_SEG_PLANES * NKEY], s_bad);
 }
-}  // namespace
-
-extern "C" int vps_pan2ch_segments(const uint8_t* pan_2ch, int H, int W, int num_stuff, uint32_t* table, uint8_t* rgb_out,
-                                   void* stream) {
+template <int KEY_CH>
+int pan2ch_segments(const uint8_t* pan_2ch, int H, int W, int num_stuff, uint32_t* table, uint8_t* rgb_out, void* stream) {
   VPS_CHECK_ARG(H >= 0 && W >= 0 && table != nullptr, "pan2ch_segments: bad arguments (H %d, W %d)", H, W);
   cudaStream_t st = (cudaStream_t)stream;
   seg_table_init_kernel<<<vps::cdiv(VPS_SEG_TABLE_WORDS, 256), 256, 0, st>>>(table);
@@ -112,14 +113,25 @@ extern "C" int vps_pan2ch_segments(const uint8_t* pan_2ch, int H, int W, int num
   const int sms = vps::num_sms();
   if (sms <= 0) { vps::set_error("pan2ch_segments: no device"); return VPS_E_NODEV; }
   const size_t smem = (size_t)VPS_SEG_PLANES * NKEY * sizeof(uint32_t);
-  cudaError_t e = cudaFuncSetAttribute(pan2ch_segments_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaError_t e = cudaFuncSetAttribute(pan2ch_segments_kernel<KEY_CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { vps::set_error("pan2ch_segments: smem attribute: %s", cudaGetErrorString(e)); return VPS_E_CUDA; }
   const bool vec = W % SEG_RUN == 0 && ((uintptr_t)pan_2ch & 15) == 0 && ((uintptr_t)rgb_out & 15) == 0;
   const int64_t nstrip = (int64_t)H * ((W + SEG_RUN - 1) / SEG_RUN);
   // about four strips per thread, at most two resident blocks per SM (the table fills 95 KiB of shared memory)
   const int64_t want = (nstrip + 256 * 4 - 1) / (256 * 4);
   const int blocks = (int)(want < 2 * sms ? (want < 1 ? 1 : want) : 2 * sms);
-  pan2ch_segments_kernel<<<blocks, 256, smem, st>>>(pan_2ch, H, W, (uint32_t)num_stuff, table, rgb_out, vec);
+  pan2ch_segments_kernel<KEY_CH><<<blocks, 256, smem, st>>>(pan_2ch, H, W, (uint32_t)num_stuff, table, rgb_out, vec);
   VPS_CUDA_LAST("pan2ch_segments");
   return VPS_OK;
+}
+}  // namespace
+
+extern "C" int vps_pan2ch_segments(const uint8_t* pan_2ch, int H, int W, int num_stuff, uint32_t* table, uint8_t* rgb_out,
+                                   void* stream) {
+  return pan2ch_segments<2>(pan_2ch, H, W, num_stuff, table, rgb_out, stream);
+}
+
+extern "C" int vps_pan2ch_image_segments(const uint8_t* pan_2ch, int H, int W, int num_stuff, uint32_t* table,
+                                         uint8_t* rgb_out, void* stream) {
+  return pan2ch_segments<1>(pan_2ch, H, W, num_stuff, table, rgb_out, stream);
 }

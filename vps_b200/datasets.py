@@ -1,5 +1,6 @@
 """The Cityscapes-VPS test split as the reference's loader walks it (mmdet/datasets/cityscapes_vps.py, custom.py, coco.py,
-pipelines/loading.py), and a small ordered prefetcher for host decoding.
+pipelines/loading.py), the Cityscapes test split of the image panoptic model (mmdet/datasets/cityscapes.py,
+`CityscapesTestSet`), and a small ordered prefetcher for host decoding.
 
 Order: the images of the annotation file (`im_all_info_{val,test}_city_vps.json`) in file order, as pycocotools' COCO keeps
 them (one entry per image id).  Reference frame (`prepare_test_img`, cityscapes_vps.py:137-148): the previous image of the
@@ -46,39 +47,38 @@ def rewrite_mode(test_cfg, mode):
     return out
 
 
-class CityscapesVPSTestSet:
-    """Test-mode CityscapesVPSDataset: `len(ds)`, `ds.img_info(i)` (with ref_id / ref_filename), `ds.paths(i)` (image and
-    reference-image paths) and `ds.img_meta(i, stage, shape)`."""
+def coco_images(ann_file):
+    """the images of a COCO-style annotation file as mmdet's CocoDataset lists them in test mode (coco.py): file order, one
+    entry per image id (pycocotools' COCO(ann_file).imgs keeps an id's first position and its last entry), with
+    filename = file_name"""
+    with open(ann_file) as f:
+        images = json.load(f)["images"]
+    by_id = {}
+    for im in images:
+        by_id[im["id"]] = im
+    return [dict(im, filename=im["file_name"]) for im in by_id.values()]
 
-    def __init__(self, ann_file, img_prefix, ref_prefix, nframes_span_test=6, data_root=None, **_):
+
+class _TestSet:
+    """`len(ds)`, `ds.img_info(i)` (with ref_filename), `ds.paths(i)` (image and reference-image paths) and
+    `ds.img_meta(i, stage, shape)` of a test-mode dataset; subclasses set the reference-frame rule in img_info"""
+
+    def __init__(self, ann_file, img_prefix, ref_prefix, data_root=None, **_):
         if data_root is not None:                                   # custom.py:57-69
             join = lambda p: p if p is None or osp.isabs(p) else osp.join(data_root, p)
             ann_file, img_prefix, ref_prefix = join(ann_file), join(img_prefix), join(ref_prefix)
         if ref_prefix is None:
             raise ValueError("ref_prefix must be specified.")
         self.ann_file, self.img_prefix, self.ref_prefix = ann_file, img_prefix, ref_prefix
-        self.nframes_span_test = int(nframes_span_test)
-        with open(ann_file) as f:
-            images = json.load(f)["images"]
-        by_id = {}
-        for im in images:                                          # COCO(ann_file).imgs: first position, last entry
-            by_id[im["id"]] = im
-        self.img_infos = [dict(im, filename=im["file_name"]) for im in by_id.values()]
+        self.img_infos = coco_images(ann_file)
 
     @classmethod
     def from_cfg(cls, test_cfg):
-        """from cfg.data.test (after rewrite_mode)"""
+        """from cfg.data.test"""
         return cls(**{k: v for k, v in test_cfg.items() if k not in ("type", "pipeline", "test_mode")})
 
     def __len__(self):
         return len(self.img_infos)
-
-    def img_info(self, idx):
-        info = dict(self.img_infos[idx])
-        prev = self.img_infos[idx - 1] if idx % self.nframes_span_test > 0 else self.img_infos[idx]
-        info["ref_id"] = prev["id"] - 1
-        info["ref_filename"] = prev["file_name"]
-        return info
 
     def paths(self, idx):
         info = self.img_info(idx)
@@ -97,3 +97,34 @@ class CityscapesVPSTestSet:
                         img_norm_cfg=dict(mean=np.array(list(stage.mean), np.float32), std=np.array(list(stage.std), np.float32),
                                           to_rgb=stage.to_rgb))
         return meta
+
+
+class CityscapesVPSTestSet(_TestSet):
+    """Test-mode CityscapesVPSDataset (cfg.data.test after rewrite_mode)."""
+
+    def __init__(self, ann_file, img_prefix, ref_prefix, nframes_span_test=6, data_root=None, **_):
+        super().__init__(ann_file, img_prefix, ref_prefix, data_root)
+        self.nframes_span_test = int(nframes_span_test)
+
+    def img_info(self, idx):
+        info = dict(self.img_infos[idx])
+        prev = self.img_infos[idx - 1] if idx % self.nframes_span_test > 0 else self.img_infos[idx]
+        info["ref_id"] = prev["id"] - 1
+        info["ref_filename"] = prev["file_name"]
+        return info
+
+
+class CityscapesTestSet(_TestSet):
+    """Test-mode CityscapesDataset of the image panoptic model (configs/cityscapes/fuse.py; mmdet/datasets/cityscapes.py:
+    82-97): the reference frame is the file of the previous frame id, read from ref_prefix (the val_nbr directory of
+    Cityscapes' neighbouring frames).  With fid = int(filename.split('_')[-2]) and suffix = '_' + filename.split('_')[-1],
+    ref_filename = filename.replace('%06d' % fid + suffix, '%06d' % (fid - 1) + suffix) when fid >= 1, else the image
+    itself; the replace is applied to the whole filename, as the reference does."""
+
+    def img_info(self, idx):
+        info = dict(self.img_infos[idx])
+        filename = info["filename"]
+        fid = int(filename.split('_')[-2])
+        suffix = '_' + filename.split('_')[-1]
+        info["ref_filename"] = filename.replace('%06d' % fid + suffix, '%06d' % (fid - 1) + suffix) if fid >= 1 else filename
+        return info

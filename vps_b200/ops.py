@@ -606,3 +606,14 @@ def tap_gather3x3(z, out, bias, act=ACT_NONE, slope=0.1, out_scale=1.0):
     check(lib().vps_tap_gather3x3(_bt(z), _bt(out), _ptr(bias), act, C.c_float(slope), C.c_float(out_scale), stream()),
           "tap_gather3x3")
     return out
+
+
+def pan2ch_segments(pan_2ch, num_stuff, table, rgb_out=None, image=False):
+    """one frame's segment table (include/vps_b200.h): pan_2ch uint8 [H,W,3] contiguous, table int32 [VPS_SEG_TABLE_WORDS],
+    rgb_out uint8 [H,W,3] or None.  image=False keys the video converter's (semantic, track) pairs (vps_pan2ch_segments),
+    image=True the image converter's (semantic, instance rank) pairs (vps_pan2ch_image_segments, the converter of
+    tools/dataset/base_dataset.py:287-335)."""
+    fn = lib().vps_pan2ch_image_segments if image else lib().vps_pan2ch_segments
+    check(fn(_ptr(pan_2ch), int(pan_2ch.shape[0]), int(pan_2ch.shape[1]), int(num_stuff), _ptr(table), _ptr(rgb_out), stream()),
+          "pan2ch_image_segments" if image else "pan2ch_segments")
+    return table

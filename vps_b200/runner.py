@@ -38,7 +38,8 @@ class ClipRunner:
         # unify: also run get_unified_pan_result (tools/dataset/cityscapes_vps.py:162-226) on the GPU for every pair
         # (vps_b200.postproc.PanUnifier) and return the uint8 [H,W,3] image as pano_results['pan_2ch'] (host) and
         # pano_results['pan_2ch_device'] (the device tensor it was downloaded from, made on the current stream, so a consumer
-        # such as PanWriter need not upload it again); a detector without a tracker gets the image-level function
+        # such as PanWriter need not upload it again), and the device semantic map as pano_results['fcn_outputs_device'] (a
+        # fresh tensor per frame, which the mIoU evaluator reads); a detector without a tracker gets the image-level function
         # (tools/dataset/base_dataset.py:232-274)
         self.unifier = None
         if unify:
@@ -203,6 +204,7 @@ class ClipRunner:
                 p2.record_stream(self.copy)
                 r[2]["pan_2ch"] = h2
                 r[2]["pan_2ch_device"] = p2
+                r[2]["fcn_outputs_device"] = sem
             if pending is not None:
                 pending[1].synchronize()               # the previous pair's maps are on the host now
                 self._raise_if_flagged(pending[2])
