@@ -223,7 +223,8 @@ int vps_tap_gather3x3(const vps_tensor* z, const vps_tensor* out, const float* b
                       void* stream);
 /* max / avg pool (resnet.py:451, tcea_modules.py:27-28; avg = count_include_pad) */
 int vps_pool2d(const vps_tensor* src, const vps_tensor* out, int k, int s, int p, int is_avg, void* stream);
-/* GroupNorm(groups, eps) + optional ReLU (upsnetFPN.py:42-51) */
+/* GroupNorm(groups, eps) + optional ReLU (upsnetFPN.py:42-51).  groups in [1, 64], c % groups == 0, c <= 1024,
+ * n * groups <= 2048 (VPS_E_ARG otherwise, nothing launched).  Deterministic: the statistics are merged in a fixed order. */
 int vps_groupnorm(const vps_tensor* x, const vps_tensor* y, const float* gamma, const float* beta, int groups,
                   float eps, int relu, void* stream);
 

@@ -2,6 +2,8 @@
 // One thread per output element with the channel index fastest => coalesced, 128-bit where the
 // channel count allows.  Torch semantics are reproduced exactly where index arithmetic matters
 // (align_corners=False bilinear, floor nearest, adaptive pooling windows).
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace {
@@ -137,132 +139,209 @@ __global__ void space_to_depth2_bf16x8_kernel(vps::TV<const __nv_bfloat16> x, vp
   *reinterpret_cast<uint4*>(y.p + y.off(n, Y, X) + k0) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
 }
 
-// ---- GroupNorm: pass 1 = per-(n,group) sum / sumsq in double via block partials; pass 2 = apply
+// ---- GroupNorm: pass 1 = per-block partial statistics of every (n, group); pass 2 = one block per (n, group) merges them
+// into mean / rstd; pass 3 = apply.  A thread keeps a running (count, mean, M2) in fp32 of x - shift, shift = the first value
+// it reads: a constant group gives mean = shift and M2 = 0 exactly, and x - shift stays exact where the mean dwarfs the
+// spread.  Partials are merged with Chan's formula in fp64 in a fixed order (no atomics), so the result does not depend on
+// the order in which blocks finish.
+struct GnPart {
+  double n, mean, m2;
+};
+
+// a <- a merged with b (Chan et al.); an empty b leaves a as it is, an empty a becomes b
+__device__ __forceinline__ void gn_merge(GnPart& a, const GnPart& b) {
+  if (b.n == 0.0) return;
+  const double n = a.n + b.n, d = b.mean - a.mean, w = b.n / n;
+  a.mean += d * w;
+  a.m2 += b.m2 + d * d * a.n * w;
+  a.n = n;
+}
+
+// lane 0 <- the merge of the warp's 32 partials, as a fixed shuffle tree
+__device__ __forceinline__ void gn_warp_merge(GnPart& p) {
+  for (int o = 16; o > 0; o >>= 1) {
+    GnPart q;
+    q.n = __shfl_down_sync(0xffffffffu, p.n, o);
+    q.mean = __shfl_down_sync(0xffffffffu, p.mean, o);
+    q.m2 = __shfl_down_sync(0xffffffffu, p.m2, o);
+    gn_merge(p, q);
+  }
+}
+
+struct GnAcc {
+  float shift, mean, m2;   // mean and M2 of x - shift
+  int n;
+  // merges a batch of k values (x - shift) with mean bm and M2 bm2 about bm
+  __device__ __forceinline__ void push(int k, float bm, float bm2) {
+    const int n1 = n + k;
+    const float d = bm - mean, w = (float)k / (float)n1;
+    mean = fmaf(d, w, mean);
+    m2 += bm2 + d * d * (float)n * w;
+    n = n1;
+  }
+  __device__ __forceinline__ GnPart part() const {
+    GnPart p;
+    p.n = n; p.mean = (double)shift + (double)mean; p.m2 = m2;
+    return p;
+  }
+};
+
+// scalar arm: grid (P, groups, n), block (p, g, n) strides over the group's elements and writes part[(n*groups + g)*P + p]
 template <typename TI>
-__global__ void gn_stats_kernel(vps::TV<const TI> x, int groups, double* __restrict__ stats) {
-  // scalar fallback. grid: (chunks, groups, n)
+__global__ void __launch_bounds__(256) gn_stats_kernel(vps::TV<const TI> x, int groups, GnPart* __restrict__ part) {
   const int g = blockIdx.y, n = blockIdx.z;
   const int cg = x.c / groups;
   const int64_t npix = (int64_t)x.h * x.w;
   const int64_t total = npix * cg;
-  double s = 0.0, ss = 0.0;
+  GnAcc acc = {0.f, 0.f, 0.f, 0};
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(i % cg);
     const int64_t pix = i / cg;
     const float v = vps::ldf<TI>(x.p + ((int64_t)n * npix + pix) * x.cs + g * cg + c);
-    s += v; ss += (double)v * v;
+    if (acc.n == 0) acc.shift = v;
+    acc.push(1, v - acc.shift, 0.f);
   }
-  __shared__ double sh[2][32];
-  for (int o = 16; o > 0; o >>= 1) { s += __shfl_down_sync(0xffffffffu, s, o); ss += __shfl_down_sync(0xffffffffu, ss, o); }
+  // fixed-order tree: shuffles within each warp, then over the warps' partials
+  GnPart p = acc.part();
+  gn_warp_merge(p);
+  __shared__ GnPart sh[32];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  if (lane == 0) { sh[0][w] = s; sh[1][w] = ss; }
+  if (lane == 0) sh[w] = p;
   __syncthreads();
   if (w == 0) {
-    s = lane < (blockDim.x >> 5) ? sh[0][lane] : 0.0;
-    ss = lane < (blockDim.x >> 5) ? sh[1][lane] : 0.0;
-    for (int o = 16; o > 0; o >>= 1) { s += __shfl_down_sync(0xffffffffu, s, o); ss += __shfl_down_sync(0xffffffffu, ss, o); }
-    if (lane == 0) {
-      atomicAdd(stats + ((int64_t)n * groups + g) * 2, s);
-      atomicAdd(stats + ((int64_t)n * groups + g) * 2 + 1, ss);
-    }
+    p = lane < (blockDim.x >> 5) ? sh[lane] : GnPart{0.0, 0.0, 0.0};
+    gn_warp_merge(p);
+    if (lane == 0) part[((int64_t)n * groups + g) * gridDim.x + blockIdx.x] = p;
   }
 }
 
-// vector path: a thread owns one 16-byte channel chunk (V channels, <= 2 groups) and strides over pixels, so a warp
-// reads whole pixels (fully coalesced); per-chunk partials are combined across the block's pixel rows in shared memory.
-// block = (C/V chunks) x (256*V/C pixel rows); grid: (pixel slices, 1, n)
-template <typename TI, int V>
-__global__ void __launch_bounds__(256) gn_stats_vec_kernel(vps::TV<const TI> x, int groups, double* __restrict__ stats) {
+// vector arm: a thread owns one 16-byte channel chunk (V channels of one group, or of two when TWO: V == 2 * cg) and strides
+// over pixels, so a warp reads whole pixels (fully coalesced).  block = (C/V chunks) x (256*V/C pixel rows); grid (P, 1, n):
+// each block merges its rows per chunk, then its chunks per group, and writes part[(n*groups + g)*P + blockIdx.x].
+template <typename TI, int V, bool TWO>
+__global__ void __launch_bounds__(256) gn_stats_vec_kernel(vps::TV<const TI> x, int groups, GnPart* __restrict__ part) {
+  constexpr int S = TWO ? 2 : 1, VS = V / S;   // groups per chunk, channels per (chunk, group)
   const int chunks = x.c / V;
   const int rows = blockDim.x / chunks;
   const int ch = threadIdx.x % chunks, row = threadIdx.x / chunks;
   const int n = blockIdx.z;
-  const int cg = x.c / groups;
-  const int c0 = ch * V;
   const int64_t npix = (int64_t)x.h * x.w;
-  float s[2] = {0.f, 0.f}, ss[2] = {0.f, 0.f};       // fp32 partials over <= a few thousand pixels, combined in double
-  double ds[2] = {0.0, 0.0}, dss[2] = {0.0, 0.0};
-  int cnt = 0;
-  if (row < rows) {
-    // 4 independent 16-byte loads in flight per thread (one was latency bound: 1.7 TB/s on an L2/HBM-resident map)
-    constexpr int U = 4;
-    const int64_t stride = (int64_t)gridDim.x * rows;
-    for (int64_t pix = (int64_t)blockIdx.x * rows + row; pix < npix; pix += U * stride) {
-      float v[U][V];
+  GnAcc acc[S];
 #pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int64_t q = pix + u * stride;
-        if (q < npix) vps::ldv<TI, V>(x.p + ((int64_t)n * npix + q) * x.cs + c0, v[u]);
-        else {
+  for (int s = 0; s < S; ++s) acc[s] = GnAcc{0.f, 0.f, 0.f, 0};
+  // 4 independent 16-byte loads in flight per thread (one was latency bound: 1.7 TB/s on an L2/HBM-resident map)
+  constexpr int U = 4;
+  const int64_t stride = (int64_t)gridDim.x * rows;
+  for (int64_t pix = (int64_t)blockIdx.x * rows + row; pix < npix; pix += U * stride) {
+    float v[U][V];
+    int k = 0;                                       // loads in range: a prefix of the U
 #pragma unroll
-          for (int j = 0; j < V; ++j) v[u][j] = 0.f;
-        }
-      }
+    for (int u = 0; u < U; ++u) {
+      const int64_t q = pix + u * stride;
+      if (q < npix) {
+        vps::ldv<TI, V>(x.p + ((int64_t)n * npix + q) * x.cs + ch * V, v[u]);
+        ++k;
+      } else {
 #pragma unroll
-      for (int u = 0; u < U; ++u) {
-#pragma unroll
-        for (int j = 0; j < V; ++j) {
-          const int gi = (V > 1 && j >= cg) ? 1 : 0;          // cg < V only when V == 2 * cg (no runtime division)
-          s[gi] += v[u][j];
-          ss[gi] += v[u][j] * v[u][j];
-        }
-      }
-      if (++cnt == 16) {
-        ds[0] += s[0]; ds[1] += s[1]; dss[0] += ss[0]; dss[1] += ss[1];
-        s[0] = s[1] = ss[0] = ss[1] = 0.f; cnt = 0;
+        for (int j = 0; j < V; ++j) v[u][j] = 0.f;
       }
     }
-    ds[0] += s[0]; ds[1] += s[1]; dss[0] += ss[0]; dss[1] += ss[1];
+#pragma unroll
+    for (int s = 0; s < S; ++s) {
+      if (acc[s].n == 0) acc[s].shift = v[0][s * VS];
+      float sum = 0.f;
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+#pragma unroll
+        for (int j = s * VS; j < (s + 1) * VS; ++j) {
+          v[u][j] -= acc[s].shift;
+          if (u < k) sum += v[u][j];
+        }
+      }
+      const int cnt = k * VS;
+      const float bm = sum / (float)cnt;
+      float bm2 = 0.f;
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+#pragma unroll
+        for (int j = s * VS; j < (s + 1) * VS; ++j) {
+          const float e = v[u][j] - bm;
+          if (u < k) bm2 = fmaf(e, e, bm2);
+        }
+      }
+      acc[s].push(cnt, bm, bm2);
+    }
   }
-  __shared__ double sh[256][4];
-  sh[threadIdx.x][0] = ds[0]; sh[threadIdx.x][1] = dss[0]; sh[threadIdx.x][2] = ds[1]; sh[threadIdx.x][3] = dss[1];
+  __shared__ GnPart sh[256][S];
+#pragma unroll
+  for (int s = 0; s < S; ++s) sh[threadIdx.x][s] = acc[s].part();
   __syncthreads();
   if (row == 0) {
-    double a0 = 0, a1 = 0, a2 = 0, a3 = 0;
-    for (int r = 0; r < rows; ++r) {
-      const double* p = sh[r * chunks + ch];
-      a0 += p[0]; a1 += p[1]; a2 += p[2]; a3 += p[3];
+#pragma unroll
+    for (int s = 0; s < S; ++s) {
+      GnPart a = sh[ch][s];
+      for (int r = 1; r < rows; ++r) gn_merge(a, sh[r * chunks + ch][s]);
+      sh[ch][s] = a;
     }
-    const int g0 = c0 / cg;
-    atomicAdd(stats + ((int64_t)n * groups + g0) * 2, a0);
-    atomicAdd(stats + ((int64_t)n * groups + g0) * 2 + 1, a1);
-    if (cg < V) {
-      atomicAdd(stats + ((int64_t)n * groups + g0 + 1) * 2, a2);
-      atomicAdd(stats + ((int64_t)n * groups + g0 + 1) * 2 + 1, a3);
+  }
+  __syncthreads();
+  const int g = threadIdx.x;
+  if (g < groups) {
+    GnPart a;
+    if constexpr (TWO) {
+      a = sh[g / 2][g % 2];
+    } else {
+      const int per = x.c / groups / V;             // chunks per group
+      a = sh[g * per][0];
+      for (int i = 1; i < per; ++i) gn_merge(a, sh[g * per + i][0]);
     }
+    part[((int64_t)n * groups + g) * gridDim.x + blockIdx.x] = a;
+  }
+}
+
+// grid (groups, n): merges the P partials of one (n, group) in a fixed order; mean and rstd are each rounded once to fp32
+__global__ void __launch_bounds__(128) gn_finalize_kernel(const GnPart* __restrict__ part, int P, float eps,
+                                                          float2* __restrict__ stats) {
+  const int64_t ng = (int64_t)blockIdx.y * gridDim.x + blockIdx.x;
+  GnPart a = {0.0, 0.0, 0.0};
+  for (int p = threadIdx.x; p < P; p += blockDim.x) gn_merge(a, part[ng * P + p]);
+  __shared__ GnPart sh[128];
+  sh[threadIdx.x] = a;
+  __syncthreads();
+  for (int s = 64; s > 0; s >>= 1) {
+    if (threadIdx.x < s) {
+      a = sh[threadIdx.x];
+      gn_merge(a, sh[threadIdx.x + s]);
+      sh[threadIdx.x] = a;
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const double var = fmax(a.m2 / a.n, 0.0);       // biased, clamped at 0 as torch does
+    stats[ng] = make_float2((float)a.mean, (float)(1.0 / sqrt(var + (double)eps)));
   }
 }
 
 constexpr int GN_MAX_C = 1024;
-// mean / rstd of every (n, group) are finalised ONCE per block into shared memory (fp64 divides per element made this
-// kernel ALU-bound); the per-element expression (v - mean) * rstd * gamma + beta is unchanged.
+// the group's mean / rstd are copied per channel into shared memory once per block, so the element loop needs no group
+// index; per-element global loads of gamma / beta made this kernel LSU-bound
 template <typename TI, typename TO, int V>
-__global__ void gn_apply_kernel(vps::TV<const TI> x, vps::TV<TO> y, const double* __restrict__ stats,
-                                const float* __restrict__ gamma, const float* __restrict__ beta, int groups, float eps,
-                                int relu) {
-  __shared__ float s_mean[64], s_rstd[64];
-  __shared__ float s_gamma[GN_MAX_C], s_beta[GN_MAX_C];      // per-element global loads of gamma/beta made this LSU-bound
+__global__ void gn_apply_kernel(vps::TV<const TI> x, vps::TV<TO> y, const float2* __restrict__ stats,
+                                const float* __restrict__ gamma, const float* __restrict__ beta, int groups, int relu) {
+  __shared__ float s_mean[GN_MAX_C], s_rstd[GN_MAX_C], s_gamma[GN_MAX_C], s_beta[GN_MAX_C];
   const int cg = x.c / groups;
-  for (int c = threadIdx.x; c < x.c; c += blockDim.x) { s_gamma[c] = gamma[c]; s_beta[c] = beta[c]; }
-  {
-    const int n_blk = blockIdx.z;                    // pix_grid: z = image index
-    const double cnt = (double)x.h * x.w * cg;
-    for (int g = threadIdx.x; g < groups; g += blockDim.x) {
-      const double m = stats[((int64_t)n_blk * groups + g) * 2] / cnt;
-      const double var = stats[((int64_t)n_blk * groups + g) * 2 + 1] / cnt - m * m;
-      s_mean[g] = (float)m;
-      s_rstd[g] = rsqrtf((float)var + eps);
-    }
+  const float2* st = stats + (int64_t)blockIdx.z * groups;      // pix_grid: z = image index
+  for (int c = threadIdx.x; c < x.c; c += blockDim.x) {
+    const float2 mr = st[c / cg];
+    s_mean[c] = mr.x; s_rstd[c] = mr.y; s_gamma[c] = gamma[c]; s_beta[c] = beta[c];
   }
   __syncthreads();
   VPS_PIX_COORDS(y, V, c, xx, yy, n);
   float v[V];
   vps::ldv<TI, V>(x.p + x.off(n, yy, xx) + c, v);
-  const int g0 = c / cg;
 #pragma unroll
   for (int j = 0; j < V; ++j) {
-    const int g = (V > 1 && cg < V) ? g0 + (j >= cg ? 1 : 0) : (cg % V == 0 ? g0 : (c + j) / cg);
-    float o = (v[j] - s_mean[g]) * s_rstd[g] * s_gamma[c + j] + s_beta[c + j];
+    const float o = (v[j] - s_mean[c + j]) * s_rstd[c + j] * s_gamma[c + j] + s_beta[c + j];
     v[j] = relu ? fmaxf(o, 0.f) : o;
   }
   vps::stv<TO, V>(y.p + y.off(n, yy, xx) + c, v);
@@ -396,48 +475,59 @@ extern "C" int vps_pool2d(const vps_tensor* src, const vps_tensor* out, int k, i
   return VPS_OK;
 }
 
-// statistics scratch: a ring of slots, one per call, so GroupNorm calls on parallel streams / graph branches never share one
-namespace { double* g_gn_ring = nullptr; unsigned g_gn_next = 0; constexpr int GN_SLOTS = 16; constexpr int GN_SLOT_DOUBLES = 4096; }
+// statistics scratch: a ring of slots, one per call, so GroupNorm calls on parallel streams / graph branches never share one.
+// A slot holds the block partials of every (n, group) and their merged (mean, rstd).
+namespace {
+constexpr int GN_SLOTS = 16, GN_MAX_NG = 2048, GN_SLOT_PARTS = 32768;
+struct GnSlot {
+  GnPart part[GN_SLOT_PARTS];
+  float2 stats[GN_MAX_NG];
+};
+GnSlot* g_gn_ring = nullptr;
+unsigned g_gn_next = 0;
+}  // namespace
 
 extern "C" int vps_groupnorm(const vps_tensor* x, const vps_tensor* y, const float* gamma, const float* beta,
                              int groups, float eps, int relu, void* stream) {
-  VPS_CHECK_ARG(x->c % groups == 0 && x->c == y->c && x->h == y->h && x->w == y->w, "groupnorm: shape");
   VPS_CHECK_ARG(groups >= 1 && groups <= 64 && x->c <= GN_MAX_C, "groupnorm: groups %d not in [1, 64] or c %d > %d", groups, x->c, GN_MAX_C);
+  VPS_CHECK_ARG(x->c % groups == 0 && x->c == y->c && x->h == y->h && x->w == y->w && x->n == y->n, "groupnorm: shape");
+  const int64_t ng = (int64_t)x->n * groups;
+  VPS_CHECK_ARG(ng <= GN_MAX_NG, "groupnorm: n * groups too large (%lld)", (long long)ng);
   const int64_t total = (int64_t)x->n * x->h * x->w * x->c;
   if (!total) return VPS_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const int64_t need = (int64_t)x->n * groups * 2;
-  VPS_CHECK_ARG(need <= GN_SLOT_DOUBLES, "groupnorm: n * groups too large (%lld)", (long long)need);
-  if (!g_gn_ring && cudaMalloc(&g_gn_ring, sizeof(double) * GN_SLOTS * GN_SLOT_DOUBLES) != cudaSuccess) {
+  if (!g_gn_ring && cudaMalloc(&g_gn_ring, sizeof(GnSlot) * GN_SLOTS) != cudaSuccess) {
     vps::set_error("groupnorm: malloc");
     return VPS_E_CUDA;
   }
-  double* g_gn_stats = g_gn_ring + (size_t)(g_gn_next++ % GN_SLOTS) * GN_SLOT_DOUBLES;
-  cudaMemsetAsync(g_gn_stats, 0, need * sizeof(double), st);
-  const int64_t per_group = (int64_t)x->h * x->w * (x->c / groups);
-  int chunks = (int)((per_group + 256 * 32 - 1) / (256 * 32));
-  if (chunks > 64) chunks = 64;
-  if (chunks < 1) chunks = 1;
+  GnSlot* slot = g_gn_ring + g_gn_next++ % GN_SLOTS;
+  const int max_parts = (int)(GN_SLOT_PARTS / ng);    // partials per (n, group) the slot has room for (>= 16)
   const int cg = x->c / groups;
+  int P;
   VPS_DISPATCH_T(x->dtype, TI, {
     constexpr int V = vps::VecW<TI>::value;
-    if (vps::vec_ok(*x, x->c) && (x->c / V) <= 256 && 256 % (x->c / V) == 0 && (cg >= V ? cg % V == 0 : V == 2 * cg)) {
-      const int rows = 256 / (x->c / V);
+    const int chunks = x->c / V;
+    if (vps::vec_ok(*x, x->c) && chunks <= 256 && 256 % chunks == 0 && (cg % V == 0 || V == 2 * cg)) {
+      const int rows = 256 / chunks;
       int64_t slices = ((int64_t)x->h * x->w + rows * 32 - 1) / (rows * 32);
       if (slices > 148 * 4) slices = 148 * 4;
-      if (slices < 1) slices = 1;
-      dim3 grid((unsigned)slices, 1, x->n);
-      gn_stats_vec_kernel<TI, V><<<grid, 256, 0, st>>>(vps::tv<const TI>(*x), groups, g_gn_stats);
+      P = (int)std::min<int64_t>(slices, max_parts);
+      const dim3 grid((unsigned)P, 1, x->n);
+      if (V == 2 * cg) gn_stats_vec_kernel<TI, V, true><<<grid, 256, 0, st>>>(vps::tv<const TI>(*x), groups, slot->part);
+      else gn_stats_vec_kernel<TI, V, false><<<grid, 256, 0, st>>>(vps::tv<const TI>(*x), groups, slot->part);
     } else {
-      dim3 grid(chunks, groups, x->n);
-      gn_stats_kernel<TI><<<grid, 256, 0, st>>>(vps::tv<const TI>(*x), groups, g_gn_stats);
+      const int64_t per_group = (int64_t)x->h * x->w * cg;
+      P = (int)std::min<int64_t>(std::min<int64_t>((per_group + 256 * 32 - 1) / (256 * 32), 64), max_parts);
+      gn_stats_kernel<TI><<<dim3(P, groups, x->n), 256, 0, st>>>(vps::tv<const TI>(*x), groups, slot->part);
     }
   });
   VPS_CUDA_LAST("gn_stats");
+  gn_finalize_kernel<<<dim3(groups, x->n), 128, 0, st>>>(slot->part, P, eps, slot->stats);
+  VPS_CUDA_LAST("gn_finalize");
   const bool vec = vps::vec_ok(*x, x->c) && vps::vec_ok(*y, x->c);
   VPS_DISPATCH_IN_OUT_V(x->dtype, y->dtype, vec, TI, TO, V,
                         (gn_apply_kernel<TI, TO, V><<<vps::pix_grid(y->w, y->c / V, y->h, y->n), 256, 0, st>>>(
-                            vps::tv<const TI>(*x), vps::tv<TO>(*y), g_gn_stats, gamma, beta, groups, eps, relu)));
+                            vps::tv<const TI>(*x), vps::tv<TO>(*y), slot->stats, gamma, beta, groups, relu)));
   VPS_CUDA_LAST("gn_apply");
   return VPS_OK;
 }
