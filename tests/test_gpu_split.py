@@ -1,10 +1,12 @@
 """GPU: a Cityscapes-VPS split tested and scored end to end.
  * vps_pan2ch_segments (the writer's segment table and pan_pred image) equals numpy exactly: golden unify / writer frames,
    random 1024x2048 frames, odd sizes, an unaligned source, an all-VOID frame, all 256 track values of one stuff class;
- * PanWriter.add_frame (device table) writes the same pred.json and PNGs as the host path on a model-produced clip;
+ * vps_pan2ch_segments' table through segments_from_table equals the oracle converter (oracle.writer.convert_frame);
+ * PanWriter.add_frame (device table) writes the same pred.json and PNGs as the oracle converter through add_frame_ids on
+   a model-produced clip;
  * vps_b200.eval_vpq on the golden split writes the reference's vpq-*.txt byte for byte;
- * vps_b200.test_vpq on an on-disk split writes what ClipRunner + PanUnifier + the host writer write in-process, and scores
-   VPQ 100 against ground truth made from that output (tc32, fp32; bf16 is reported)."""
+ * vps_b200.test_vpq on an on-disk split writes what ClipRunner + PanUnifier + the oracle converter write in-process, and
+   scores VPQ 100 against ground truth made from that output (tc32, fp32; bf16 is reported)."""
 import filecmp
 import json
 import os
@@ -21,8 +23,8 @@ HERE = os.path.join(os.path.dirname(__file__), "golden")
 
 
 def _check_frame(p2_np, src=None):
-    from oracle import vpq as V
-    from vps_b200.writer import PanWriter, id2rgb, pan2ch_segments, segments_from_table
+    from oracle.writer import convert_frame
+    from vps_b200.writer import id2rgb, pan2ch_segments, segments_from_table
     src = torch.from_numpy(p2_np).cuda() if src is None else src
     table, rgb = pan2ch_segments(src)
     want = _numpy_table(p2_np)
@@ -30,10 +32,9 @@ def _check_frame(p2_np, src=None):
     assert np.array_equal(table[0], want[0])
     for i in range(1, 5):
         assert np.array_equal(table[i][area], want[i][area]), i
-    ids, segs = V.segments_from_pan2ch(p2_np)
+    segs, ids = convert_frame(p2_np)
     assert np.array_equal(rgb.cpu().numpy(), id2rgb(ids))
-    ann = PanWriter(None, sample=False).add_frame_ids("f", ids, segs, p2_np)
-    assert segments_from_table(table) == ann["segments_info"]
+    assert segments_from_table(table) == segs
 
 
 def _random_frame(rng, H, W, block=16):
@@ -45,7 +46,7 @@ def _random_frame(rng, H, W, block=16):
     return out
 
 
-def test_segment_table_golden_frames(cuda):
+def test_segment_table_golden_frames_vs_oracle(cuda):
     d = np.load(os.path.join(HERE, "unify_pan.npz"))
     keys = [k for k in d.keys() if k.startswith("out")]
     assert keys
@@ -56,7 +57,7 @@ def test_segment_table_golden_frames(cuda):
         _check_frame(fr)
 
 
-def test_segment_table_random_odd_and_edge_frames(cuda):
+def test_segment_table_random_odd_and_edge_frames_vs_oracle(cuda):
     rng = np.random.default_rng(5)
     _check_frame(_random_frame(rng, 1024, 2048))
     _check_frame(_random_frame(rng, 1024, 2048, block=1))           # a run per pixel
@@ -103,8 +104,8 @@ def _same_tree(a, b):
             assert np.array_equal(np.asarray(Image.open(os.path.join(a, sub, f))), np.asarray(Image.open(os.path.join(b, sub, f))))
 
 
-def test_writer_device_table_equals_host_path(cuda, tmp_path):
-    from oracle import vpq as V
+def test_writer_device_table_equals_oracle_host_path(cuda, tmp_path):
+    from oracle.writer import convert_frame
     from vps_b200.writer import PanWriter
     clip = _model_clip("fp32")
     dev, host = PanWriter(str(tmp_path / "dev"), sample=False, workers=2, max_pending=2), PanWriter(str(tmp_path / "host"), sample=False)
@@ -117,7 +118,7 @@ def test_writer_device_table_equals_host_path(cuda, tmp_path):
         else:                                                            # device input with a host copy, as the driver
             a = dev.add_frame(name, p2.cuda(), pan_2ch_host=p2)
         p = p2.numpy()
-        assert a == host.add_frame_ids(name, *V.segments_from_pan2ch(p), p)
+        assert a == host.add_frame_ids(name, *convert_frame(p), p)
     assert dev.finish() == host.finish()
     _same_tree(str(tmp_path / "dev"), str(tmp_path / "host"))
 
@@ -126,6 +127,7 @@ def test_eval_vpq_golden_split_byte_identical(cuda, tmp_path):
     from vps_b200 import eval_vpq as E
     sub = tmp_path / "submit"
     shutil.copytree(os.path.join(GOLD, "submit"), str(sub))
+    os.chmod(str(sub), 0o755)                       # copytree keeps the mode of a read-only checkout; vpq-*.txt go here
     assert E.main(["--submit_dir", str(sub) + "/", "--truth_dir", os.path.join(GOLD, "truth"),
                    "--pan_gt_json_file", os.path.join(GOLD, "gt.json"), "--workers", "3"]) == 0
     for f in ("vpq-0.txt", "vpq-5.txt", "vpq-10.txt", "vpq-15.txt", "vpq-final.txt"):
@@ -183,8 +185,9 @@ def _write_split(root):
 
 
 def _in_process(root, images, frames, names, precision, out):
-    """ClipRunner + PanUnifier + the host writer, fed directly (frame i references frame i - 1 inside its clip)"""
-    from oracle import vpq as V
+    """ClipRunner + PanUnifier + the oracle converter + the host writer, fed directly (frame i references frame i - 1
+    inside its clip)"""
+    from oracle.writer import convert_frame
     from vps_b200 import test_vpq as T
     from vps_b200.pipeline import InputStage
     from vps_b200.runner import ClipRunner
@@ -202,7 +205,7 @@ def _in_process(root, images, frames, names, precision, out):
     for i, r in enumerate(runner.run(pairs, metas)):
         p = r[2]["pan_2ch"].numpy().copy()
         name = next(it) if i >= 4 and (i - 4) % 5 == 0 else None
-        w.add_frame_ids(name, *V.segments_from_pan2ch(p), p)
+        w.add_frame_ids(name, *convert_frame(p), p)
     return w.finish()
 
 
@@ -222,7 +225,7 @@ def _truth_from(out, names, root):
     return truth, path, pred
 
 
-def test_test_vpq_driver_whole_chain(cuda, tmp_path):
+def test_test_vpq_driver_whole_chain_vs_oracle_writer(cuda, tmp_path):
     from vps_b200 import eval_vpq as E
     from vps_b200 import test_vpq as T
     root = str(tmp_path / "cityscapes_vps")         # the tracker reads img_meta filenames under a Cityscapes path

@@ -4,7 +4,7 @@
  * the GT / prediction file-name mapping and the clip split;
  * the test dataset's order, reference frame and img_meta fields (cityscapes_vps.py:137-148, loading.py:43-67);
  * the command lines, the --mode rewrite and the stuff area limit read from the UPSNet yaml;
- * the writer's host step (key table -> segments_info) against the numpy converter."""
+ * the writer's host step (key table -> segments_info) against the oracle converter."""
 import json
 import os
 
@@ -138,19 +138,17 @@ def _numpy_table(p2):
     return t.reshape(5, 19, 256)
 
 
-def test_segments_from_table_equals_host_writer():
-    from oracle import vpq as V
+def test_segments_from_table_equals_oracle_converter():
+    from oracle.writer import convert_frame
     from tests.test_writer_cpu import _golden
-    from vps_b200.writer import PanWriter, segments_from_table
+    from vps_b200.writer import segments_from_table
     frames, _, _ = _golden()
     rng = np.random.default_rng(3)
     extra = np.zeros((20, 30, 3), np.uint8)
     extra[..., 0] = 5
     extra[..., 2] = rng.integers(0, 256, (20, 30))                 # one stuff class, many track values
     for fr in list(frames) + [extra]:
-        w = PanWriter(None, sample=False)
-        ann = w.add_frame_ids("f", *V.segments_from_pan2ch(fr), fr)
-        assert segments_from_table(_numpy_table(fr)) == ann["segments_info"]
+        assert segments_from_table(_numpy_table(fr)) == convert_frame(fr)[0]
 
 
 def test_driver_refuses_an_unsorted_split(tmp_path):

@@ -2,7 +2,7 @@
  * oracle/writer.py vs the reference's own converter_2ch_track_core (golden made by tests/golden/make_writer_golden.py with a
    stand-in colour generator): same segments (category, bbox, area) and the same pixel partition, ids modulo a bijection that
    keeps a thing's id across frames;
- * vps_b200.writer.PanWriter's host part vs the oracle exactly, PNG round trip and pred.json included."""
+ * vps_b200.writer.PanWriter's host part fed by the oracle: PNG round trip, pred.json and frame sampling."""
 import json
 import os
 
@@ -49,7 +49,7 @@ def test_oracle_matches_reference_modulo_ids():
     assert seen_multi, "golden clip must contain a stuff category with more than one key"
 
 
-def test_product_writer_host_part(tmp_path):
+def test_product_writer_host_part_fed_by_oracle(tmp_path):
     from oracle import vpq as V
     from oracle import writer as Wo
     from PIL import Image
@@ -57,19 +57,21 @@ def test_product_writer_host_part(tmp_path):
     frames, _, _ = _golden()
     names = ["frankfurt_%06d_leftImg8bit.png" % i for i in range(len(frames))]
     w = PanWriter(str(tmp_path), sample=False)
-    for name, fr in zip(names, frames):
-        ids, segs = V.segments_from_pan2ch(fr)                      # numpy stand-in for the device ops
-        ann = w.add_frame_ids(name, ids, segs, fr)
-        ref_segs, ref_ids = Wo.convert_frame(fr)
-        assert np.array_equal(ids, ref_ids)
-        assert sorted(ann["segments_info"], key=lambda s: s["id"]) == sorted(ref_segs, key=lambda s: s["id"])
+    converted = [Wo.convert_frame(fr) for fr in frames]
+    for name, fr, (segs, ids) in zip(names, frames, converted):
+        v_ids, v_segs = V.segments_from_pan2ch(fr)                  # the numpy VPQ chain segments frames as the converter
+        assert np.array_equal(v_ids, ids)
+        assert v_segs == [{k: s[k] for k in ("id", "category_id", "iscrowd", "area")} for s in segs]
+        assert w.add_frame_ids(name, segs, ids, fr) == {"segments_info": segs}
+    pred = w.finish()
+    assert json.load(open(os.path.join(str(tmp_path), "pred.json"))) == pred
+    assert pred["annotations"] == [{"segments_info": segs} for segs, _ in converted]
+    for name, fr, (_, ids) in zip(names, frames, converted):
         png = np.asarray(Image.open(os.path.join(str(tmp_path), "pan_pred", name.replace("_leftImg8bit", ""))))
         assert np.array_equal(Wo.rgb2id(png), ids)
         p2 = np.asarray(Image.open(os.path.join(str(tmp_path), "pan_2ch", name.replace("_leftImg8bit", ""))))
         assert np.array_equal(p2, fr)
-    pred = w.finish()
-    assert json.load(open(os.path.join(str(tmp_path), "pred.json"))) == pred and len(pred["annotations"]) == len(frames)
     # frame sampling of inference_panoptic_video: [(20 // 5)::5]
     w2 = PanWriter(None)
-    kept = [i for i in range(30) if w2.add_frame_ids("f%d" % i, *V.segments_from_pan2ch(frames[0])) is not None]
+    kept = [i for i in range(30) if w2.add_frame_ids("f%d" % i, *converted[0], frames[0]) is not None]
     assert kept == list(range(30))[4::5]

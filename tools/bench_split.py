@@ -1,9 +1,8 @@
 """Benchmark of the split-level tools (vps_b200.test_vpq, vps_b200.eval_vpq) on one GPU; prints one JSON line.
 
-  writer     per sampled 1024x2048 frame: the previous host writer (device ids + pair table, then last_key_ids,
-             find_objects, id2rgb and two serial PNG encodes), PanWriter.add_frame (device segment table, PNGs on writer
-             threads; timed over a run of frames up to finish()), the same without PNGs, and vps_pan2ch_segments alone
-             (CUDA events over many launches; algorithmic bytes = 6 MB read + 6 MB written)
+  writer     per sampled 1024x2048 frame: PanWriter.add_frame (device segment table, PNGs on writer threads; timed over a
+             run of frames up to finish()), the same without PNGs, and vps_pan2ch_segments alone (CUDA events over many
+             launches; algorithmic bytes = 6 MB read + 6 MB written)
   eval       vps_b200.vpq.evaluate_split per frame on decoded 1024x2048 frames (PNG decode excluded), 12 frames, 4 windows
   driver     vps_b200.test_vpq.run_split on a synthetic on-disk split (2 clips x 30 frames of 1024x2048, seeded test weights)
              in frames/s, against ClipRunner(unify=True) on the same frames already decoded in memory (the model-only rate)
@@ -48,30 +47,17 @@ def synth_pan2ch(rng, H=1024, W=2048):
     return out
 
 
-def old_add_frame(w, name, pan_2ch):
-    """the previous PanWriter.add_frame: device ids and pair table, then the host part with serial PNG encodes"""
-    from vps_b200.vpq import segments_from_pan2ch
-    from vps_b200.writer import last_key_ids
-    ids, segs = segments_from_pan2ch(pan_2ch)
-    p2 = pan_2ch.cpu().numpy()
-    return w.add_frame_ids(name, ids.cpu().numpy().astype(np.uint32), segs, p2, _counted=True, bbox_ids=last_key_ids(p2))
-
-
 def bench_writer(frames, tmp):
     from vps_b200.writer import PanWriter, pan2ch_segments
     dev = [torch.from_numpy(f).cuda() for f in frames]
     names = ["frankfurt_%06d_leftImg8bit.png" % i for i in range(len(frames))]
     out = {}
     # warm-up
-    old_add_frame(PanWriter(os.path.join(tmp, "w0"), sample=False), names[0], dev[0])
+    w = PanWriter(os.path.join(tmp, "w0"), sample=False)
+    w.add_frame(names[0], dev[0])
+    w.finish()
     PanWriter(None, sample=False).add_frame(names[0], dev[0])
     torch.cuda.synchronize()
-    w = PanWriter(os.path.join(tmp, "old"), sample=False)
-    t = time.perf_counter()
-    for n, d in zip(names, dev):
-        old_add_frame(w, n, d)
-    w.finish()
-    out["old_add_frame_ms"] = 1e3 * (time.perf_counter() - t) / len(frames)
     w = PanWriter(os.path.join(tmp, "new"), sample=False)
     t = time.perf_counter()
     for n, d in zip(names, dev):

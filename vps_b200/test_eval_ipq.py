@@ -22,7 +22,6 @@ PNGs are id2rgb of deterministic ids rather than random panopticapi colours; and
 panoptic GT json (the reference pairs the sorted predictions with the json's images by position and silently mispairs, or
 drops unreadable GT files): a split that does not pair raises ValueError before the model runs."""
 import argparse
-import itertools
 import json
 import os
 import re
@@ -200,37 +199,12 @@ class SplitScorer:
 
 def run_split(cfg, model, dataset, helper, out, area_limit=4096, workers=4, device="cuda:0"):
     """single_gpu_test + get_unified_pan_result + evaluate_ssegs + evaluate_panoptic over a whole split"""
-    import cv2
-    import torch
-
-    from .datasets import prefetch_map
-    from .pipeline import InputStage
-    from .runner import ClipRunner
+    from .test_vpq import run_frames
     names = [dataset.img_info(i)["filename"].split("/")[-1] for i in range(len(dataset))]
     helper.pair(names)                                          # before the model runs
-    stage = InputStage.from_pipeline(cfg.data.test.pipeline, device=device)
-    with_ref = model.with_flow
-
-    def read(idx):
-        img_path, ref_path = dataset.paths(idx)
-        img = cv2.imread(img_path, cv2.IMREAD_COLOR)
-        if img is None:
-            raise FileNotFoundError(img_path)
-        ref = None
-        if with_ref:
-            ref = cv2.imread(ref_path, cv2.IMREAD_COLOR)
-            if ref is None:
-                raise FileNotFoundError(ref_path)
-        pair = (torch.from_numpy(img), None if ref is None else torch.from_numpy(ref))
-        return pair, dataset.img_meta(idx), helper.load_gt(idx)
-
-    a, b, c = itertools.tee(prefetch_map(read, range(len(dataset)), workers=workers, depth=8), 3)
-    pairs, metas, gts = (x[0] for x in a), (x[1] for x in b), (x[2] for x in c)
-    runner = ClipRunner(model, device, unify=True, input_stage=stage)
-    runner.unifier.stuff_area_limit = int(area_limit)
+    frames = run_frames(cfg, model, dataset, area_limit, workers, device, extra=helper.load_gt)
     with SplitScorer(helper, out, workers) as scorer:
-        for name, r, gt in zip(names, runner.run(pairs, metas), gts):
-            p = r[2]
+        for name, (p, gt) in zip(names, frames):
             scorer.add(name, p["fcn_outputs_device"], p["pan_2ch_device"], p["fcn_outputs"], p["pan_2ch"], gt)
         return scorer.finish()
 

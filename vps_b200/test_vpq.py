@@ -71,27 +71,19 @@ def load_model(config, checkpoint, device, precision):
     return cfg, model
 
 
-def run_split(cfg, model, dataset, names, output_dir, area_limit=4096, workers=4, device="cuda:0"):
-    """the loop of single_gpu_test + get_unified_pan_result + inference_panoptic_video over a whole split; returns pred.json"""
+def run_frames(cfg, model, dataset, area_limit=4096, workers=4, device="cuda:0", extra=None):
+    """single_gpu_test + get_unified_pan_result over the dataset's frames in order: each (image, reference) pair is decoded
+    with cv2 and given its img_meta on `workers` threads a few frames ahead of the model, which runs in a
+    `ClipRunner(unify=True)` with the stuff area limit.  The runner is built here; the returned iterator yields
+    (pano_results, extra(idx)) per frame.  `extra`, when given, runs on the decode threads too; without it the second
+    element is None."""
     import cv2
     import torch
 
+    from .datasets import prefetch_map
     from .pipeline import InputStage
     from .runner import ClipRunner
-    from .writer import PanWriter
     stage = InputStage.from_pipeline(cfg.data.test.pipeline, device=device)
-    # the reference keys the unified results by file basename and sorts them before sampling (test_vpq.py:170-176); the
-    # frames run in dataset order, so the two orders must agree (they do for Cityscapes-VPS names)
-    base = [dataset.img_info(i)["filename"].split("/")[-1] for i in range(len(dataset))]
-    if base != sorted(set(base)):
-        raise ValueError("the dataset's images are not in ascending, unique file-name order: the reference samples the "
-                         "sorted results, which this driver does not reorder")
-    writer = PanWriter(output_dir, workers=workers)
-    sampled = list(range(len(dataset)))[writer.start::writer.step]
-    if len(sampled) != len(names):
-        raise ValueError("%d frames are sampled from %d images but the pan_im_json lists %d names"
-                         % (len(sampled), len(dataset), len(names)))
-    name_of = dict(zip(sampled, names))
     with_ref = model.with_flow
 
     def read(idx):
@@ -105,17 +97,35 @@ def run_split(cfg, model, dataset, names, output_dir, area_limit=4096, workers=4
             if ref is None:
                 raise FileNotFoundError(ref_path)
         pair = (torch.from_numpy(img), None if ref is None else torch.from_numpy(ref))
-        return pair, dataset.img_meta(idx)
+        return pair, dataset.img_meta(idx), None if extra is None else extra(idx)
 
-    from .datasets import prefetch_map
-    a, b = itertools.tee(prefetch_map(read, range(len(dataset)), workers=workers, depth=8))   # zip below keeps them in step
-    pairs, metas = (pair for pair, _ in a), (meta for _, meta in b)
+    # the runner reads a frame or two ahead of what it yields; tee holds the extras until their frame comes out
+    a, b, c = itertools.tee(prefetch_map(read, range(len(dataset)), workers=workers, depth=8), 3)
     runner = ClipRunner(model, device, unify=True, input_stage=stage)
     runner.unifier.stuff_area_limit = int(area_limit)
+    return zip((r[2] for r in runner.run((x[0] for x in a), (x[1] for x in b))), (x[2] for x in c))
+
+
+def run_split(cfg, model, dataset, names, output_dir, area_limit=4096, workers=4, device="cuda:0"):
+    """the loop of single_gpu_test + get_unified_pan_result + inference_panoptic_video over a whole split; returns pred.json"""
+    from .writer import PanWriter
+    # the reference keys the unified results by file basename and sorts them before sampling (test_vpq.py:170-176); the
+    # frames run in dataset order, so the two orders must agree (they do for Cityscapes-VPS names)
+    base = [dataset.img_info(i)["filename"].split("/")[-1] for i in range(len(dataset))]
+    if base != sorted(set(base)):
+        raise ValueError("the dataset's images are not in ascending, unique file-name order: the reference samples the "
+                         "sorted results, which this driver does not reorder")
+    writer = PanWriter(output_dir, workers=workers)
+    sampled = list(range(len(dataset)))[writer.start::writer.step]
+    if len(sampled) != len(names):
+        raise ValueError("%d frames are sampled from %d images but the pan_im_json lists %d names"
+                         % (len(sampled), len(dataset), len(names)))
+    name_of = dict(zip(sampled, names))
+    frames = run_frames(cfg, model, dataset, area_limit, workers, device)
     model.reset_tracker()
     with writer:
-        for idx, r in enumerate(runner.run(pairs, metas)):
-            writer.add_frame(name_of.get(idx), r[2]["pan_2ch_device"], pan_2ch_host=r[2]["pan_2ch"])
+        for idx, (p, _) in enumerate(frames):
+            writer.add_frame(name_of.get(idx), p["pan_2ch_device"], pan_2ch_host=p["pan_2ch"])
         return writer.finish()
 
 
